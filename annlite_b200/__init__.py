@@ -1,4 +1,4 @@
-"""annlite_b200: B200-native PQ-ADC / PQ-HNSW search path behind AnnLite's Python surface."""
+"""annlite_b200: H100-native (sm_90a) PQ-ADC / PQ-HNSW search path behind AnnLite's Python surface."""
 from .enums import ExpandMode, Metric  # noqa: F401
 
 __all__ = ['AnnLite', 'HnswIndex', 'PQIndex', 'PQCodec', 'Metric', 'ExpandMode', 'Engine']

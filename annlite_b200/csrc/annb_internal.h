@@ -152,7 +152,7 @@ struct annb_index {
   int device = 0;
   int metric = ANNB_METRIC_L2;
   int dim = 0, M = 0, Ks = 0, ds = 0, code_bytes = 1;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;  // second lane of the chunked host-buffer pipeline (annb_search)
   cudaEvent_t ev[6] = {nullptr};  // [0,1] K1, [2,3] K3, [4,5] K2

@@ -1,11 +1,11 @@
 #!/usr/bin/env bash
-# Builds annlite_b200/lib/libannlite_b200.so for sm_100a (nvcc cross-compiles without a GPU).
+# Builds annlite_b200/lib/libannlite_b200.so for sm_90a (H100; nvcc cross-compiles without a GPU).
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 OUT="$HERE/../lib"
 mkdir -p "$OUT" "$HERE/obj"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-ARCH="-gencode arch=compute_100a,code=sm_100a"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
 CXXFLAGS="-O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function ${ANNB_EXTRA_NVCC:-}"
 pids=()
 for f in adc_table adc_scan hnsw_search walk_fused walk_flagged4 gpu_build capi; do

@@ -615,7 +615,7 @@ int annb_add_items(annb_index_t *h, const float *vectors, const void *codes, con
   ANNB_CUDA(cudaStreamSynchronize(h->stream));   // insertion reuses search scratch: let streamed searches finish
   ANNB_CUDA(cudaStreamSynchronize(h->stream2));
   // num_threads == 1 is the reference's deterministic single-threaded build; any other value is an unordered
-  // concurrent build in the reference too -- large batches of fresh rows then take the GPU builder
+  // concurrent build in the reference too -- large batches of fresh rows then take the GPU builder (deterministic itself)
   if (num_threads != 1 && !codes && h->opt_gpu_build) {
     const int rc = gpu_build_run(h, vectors, labels, n, num_threads);
     if (rc != 1) return rc;

@@ -15,13 +15,16 @@
 //   phase 2 (device) the remaining rows, all of level 0, in batches: PQ-encode (encode_kernel), ONE launch of the
 //            search kernel itself (hnsw_walk4, table built in shared memory from the row's vector, ef = ef_construction,
 //            k = M_, internal ids out) against the graph as it stood before the batch, then link_new_nodes_kernel
-//            writes the new records and reverse_link_kernel applies the back-links under a per-node spin lock,
-//            evaluating "closer to x than r" directly from x's vector and the codebook with the table's arithmetic.
+//            writes the new records and reverse_link_kernel applies the back-links, one warp per neighbour r taking
+//            r's back-links in row order, evaluating "closer to x than r" directly from x's vector and the codebook
+//            with the table's arithmetic.
 //   finish   links and codes are exported, the host graph (reference byte layout: save_index, pickle state,
 //            mark_deleted, further add_items all keep working) is assembled from them.
 //
 // Rows of one batch do not see each other as candidates (the multi-threaded reference has the same kind of race:
 // concurrent insertions see a partially linked graph); batches grow with the graph (<= 1/16 of it by default, <= 65536 rows).
+// The result is deterministic: phase 1 inserts on one host thread and phase 2 fixes the order of every write, so the
+// same rows give the same graph on every run and machine, whatever num_threads is.
 // The graph is NOT the one a sequential build makes; what is checked is what matters for the path: every structural
 // invariant (HostGraph::validate), oracle parity of searches over the result, and recall against a host-built
 // graph of the same data (tests/test_gpu_build.py).
@@ -68,7 +71,6 @@ struct BuildDev {
   uint8_t *rec0;           // level-0 walk records (mutable)
   uint64_t *labels;        // by internal id
   uint8_t *node_codes;     // (N, M) own code of every node
-  int *locks;              // (N) spin locks
   int rec0_bytes, code_off0, maxM0, M;
 };
 
@@ -97,65 +99,62 @@ __global__ void link_new_nodes_kernel(BuildDev b, const uint64_t *__restrict__ s
   if (lane == 0) b.labels[x] = new_labels[i];
 }
 
-// back-links: one warp per (new node x, selected neighbour r) pair, r's record updated under r's lock
-__global__ void reverse_link_kernel(BuildDev b, const uint64_t *__restrict__ sel, const float *__restrict__ seld,
-                                    const int32_t *__restrict__ found, int k, const float *__restrict__ q, int dim,
-                                    const float *__restrict__ cb, int ds, int is_ip, float bias, uint32_t first, int B) {
-  const int64_t p = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+// back-links: one warp per neighbour r selected in this batch, applying r's back-links one after the other in row
+// order (pairs p = i*k + j ascending, as a sequential insertion of the batch would): the graph a batch leaves does not
+// depend on the order in which warps run.  rows / off / pairs: the host's counting sort of the batch's (r, p) pairs.
+__global__ void reverse_link_kernel(BuildDev b, const uint32_t *__restrict__ rows, const uint32_t *__restrict__ off,
+                                    const uint32_t *__restrict__ pairs, int R, const float *__restrict__ seld, int k,
+                                    const float *__restrict__ q, int dim, const float *__restrict__ cb, int ds, int is_ip,
+                                    float bias, uint32_t first) {
+  const int w = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
-  if (p >= (int64_t)B * k) return;
-  const int i = (int)(p / k), j = (int)(p - (int64_t)i * k);
-  if (j >= min(found[i], k)) return;
-  const uint32_t r = (uint32_t)sel[p];
-  const uint32_t x = first + i;
-  const float dr = seld[p];
+  if (w >= R) return;
+  const uint32_t r = rows[w];
   uint8_t *rec = b.rec0 + (size_t)r * b.rec0_bytes;
   volatile uint32_t *links = reinterpret_cast<volatile uint32_t *>(rec);
   volatile uint8_t *codes = rec + b.code_off0;
   const int M = b.M;
-  if (lane == 0) {
-    while (atomicCAS(b.locks + r, 0, 1) != 0) {
+  for (uint32_t e = off[w]; e < off[w + 1]; e++) {
+    const uint32_t p = pairs[e];
+    const int i = (int)(p / (uint32_t)k);
+    const uint32_t x = first + i;
+    const float dr = seld[p];
+    __syncwarp();  // the previous back-link's writes to r's record are visible to every lane
+    uint32_t link = lane < b.maxM0 ? links[lane] : EMPTY_LINK;
+    const bool valid = link != EMPTY_LINK;
+    const int cnt = __popc(__ballot_sync(FULL_MASK, valid));
+    const uint8_t *xcode = b.node_codes + (size_t)x * M;
+    if (cnt < b.maxM0) {
+      // room: append (hnswalg.h:575-578)
+      if (lane == 0) links[cnt] = x;
+      for (int t = lane; t < M; t += 32) codes[(size_t)cnt * M + t] = xcode[t];
+    } else {
+      // full: keep x and the neighbours that are not closer to x than r is; descending id, at most maxM0 (:579-616 in PQ mode)
+      uint8_t mycode[128];
+      for (int t = 0; t < M; t++) mycode[t] = valid ? codes[(size_t)lane * M + t] : 0;
+      float d = CUDART_INF_F;
+      if (valid) d = adc_direct(q + (size_t)i * dim, cb, mycode, M, ds, is_ip, bias);
+      const bool keep = valid && !(d < dr);
+      int rank = 0;
+      for (int s = 0; s < 32; s++) {
+        const uint32_t oid = __shfl_sync(FULL_MASK, link, s);
+        const bool ok = __shfl_sync(FULL_MASK, (int)keep, s);
+        rank += (ok && oid > link) ? 1 : 0;
+      }
+      const int nkeep = __popc(__ballot_sync(FULL_MASK, keep));
+      const int total = min(1 + nkeep, b.maxM0);
+      __syncwarp();  // every lane holds its old link and code in registers: the record may be rewritten
+      if (keep && 1 + rank < b.maxM0) {
+        links[1 + rank] = link;
+        for (int t = 0; t < M; t++) codes[(size_t)(1 + rank) * M + t] = mycode[t];
+      }
+      if (lane == 0) {
+        links[0] = x;
+        for (int t = 0; t < M; t++) codes[t] = xcode[t];
+      }
+      if (lane >= total && lane < b.maxM0) links[lane] = EMPTY_LINK;
     }
   }
-  __syncwarp();
-  __threadfence();
-  uint32_t link = lane < b.maxM0 ? links[lane] : EMPTY_LINK;
-  const bool valid = link != EMPTY_LINK;
-  const int cnt = __popc(__ballot_sync(FULL_MASK, valid));
-  const uint8_t *xcode = b.node_codes + (size_t)x * M;
-  if (cnt < b.maxM0) {
-    // room: append (hnswalg.h:575-578)
-    if (lane == 0) links[cnt] = x;
-    for (int t = lane; t < M; t += 32) codes[(size_t)cnt * M + t] = xcode[t];
-  } else {
-    // full: keep x and the neighbours that are not closer to x than r is; descending id, at most maxM0 (:579-616 in PQ mode)
-    uint8_t mycode[128];
-    for (int t = 0; t < M; t++) mycode[t] = valid ? codes[(size_t)lane * M + t] : 0;
-    float d = CUDART_INF_F;
-    if (valid) d = adc_direct(q + (size_t)i * dim, cb, mycode, M, ds, is_ip, bias);
-    const bool keep = valid && !(d < dr);
-    int rank = 0;
-    for (int s = 0; s < 32; s++) {
-      const uint32_t oid = __shfl_sync(FULL_MASK, link, s);
-      const bool ok = __shfl_sync(FULL_MASK, (int)keep, s);
-      rank += (ok && oid > link) ? 1 : 0;
-    }
-    const int nkeep = __popc(__ballot_sync(FULL_MASK, keep));
-    const int total = min(1 + nkeep, b.maxM0);
-    __syncwarp();  // every lane holds its old link and code in registers: the record may be rewritten
-    if (keep && 1 + rank < b.maxM0) {
-      links[1 + rank] = link;
-      for (int t = 0; t < M; t++) codes[(size_t)(1 + rank) * M + t] = mycode[t];
-    }
-    if (lane == 0) {
-      links[0] = x;
-      for (int t = 0; t < M; t++) codes[t] = xcode[t];
-    }
-    if (lane >= total && lane < b.maxM0) links[lane] = EMPTY_LINK;
-  }
-  __threadfence();
-  __syncwarp();
-  if (lane == 0) atomicExch(b.locks + r, 0);
 }
 
 // links of every node, maxM0 u32 each (0xFFFFFFFF = empty), for the host graph
@@ -209,7 +208,8 @@ int gpu_build_run(annb_index *h, const float *vectors, const uint64_t *labels, i
       l1[t] = labels[p1[t]];
       f1[t] = lv[p1[t]];
     }
-    ANNB_TRY_RC(hnsw_host_add(h, v1.data(), nullptr, l1.data(), (int64_t)p1.size(), num_threads, f1.data()));
+    // one thread: a concurrent host insertion would make the graph depend on thread timing (the build is deterministic)
+    ANNB_TRY_RC(hnsw_host_add(h, v1.data(), nullptr, l1.data(), (int64_t)p1.size(), 1, f1.data()));
   }
   const int64_t n1 = g.count.load();
   const int64_t n2 = (int64_t)p2.size();
@@ -234,9 +234,6 @@ int gpu_build_run(annb_index *h, const float *vectors, const uint64_t *labels, i
   void *p;
   ANNB_TRY_RC(annb_scratch(h, S_RAW0, (size_t)N * M, &p));  // raw upload buffer is free again after the sync
   b.node_codes = (uint8_t *)p;
-  ANNB_TRY_RC(annb_scratch(h, S_VISITED, (size_t)N * 4, &p));
-  b.locks = (int *)p;
-  ANNB_CUDA(cudaMemsetAsync(b.locks, 0, (size_t)N * 4, h->stream));
   {
     std::vector<uint8_t> c1((size_t)n1 * M);
     for (int64_t i = 0; i < n1; i++) memcpy(c1.data() + (size_t)i * M, g.code((uint32_t)i), (size_t)M);
@@ -262,6 +259,11 @@ int gpu_build_run(annb_index *h, const float *vectors, const uint64_t *labels, i
   uint64_t *hlab;
   ANNB_TRY_RC(annb_pinned(h, 0, (size_t)BMAX * dim * 4, (void **)&hq));
   ANNB_TRY_RC(annb_pinned(h, 1, (size_t)BMAX * 8, (void **)&hlab));
+  uint32_t *dcsr;  // a batch's back-links grouped by neighbour: [off (R+1)][rows (R)][pairs (P)]
+  ANNB_TRY_RC(annb_scratch(h, S_CAND, ((size_t)3 * BMAX * k + 1) * 4, (void **)&dcsr));
+  std::vector<uint64_t> hsel((size_t)BMAX * k);
+  std::vector<int32_t> hfound((size_t)BMAX);
+  std::vector<uint32_t> cnt((size_t)N), pos((size_t)N), hrows, hoff, hpairs;
   const int is_ip = h->metric != ANNB_METRIC_L2;
   const float bias = h->opt_ip_raw ? 0.f : (float)(1.0 / (double)h->Ks);
   int64_t n_cur = n1, done = 0;
@@ -296,8 +298,38 @@ int gpu_build_run(annb_index *h, const float *vectors, const uint64_t *labels, i
     if (rc) return rc;
     const unsigned wb = 8;  // warps per block
     link_new_nodes_kernel<<<(unsigned)((B + wb - 1) / wb), wb * 32, 0, h->stream>>>(b, dsel, dfound, k, dlab, (uint32_t)n_cur, (int)B);
-    reverse_link_kernel<<<(unsigned)((B * k + wb - 1) / wb), wb * 32, 0, h->stream>>>(b, dsel, dseld, dfound, k, dq, dim, h->d_codebook,
-                                                                                    h->ds, is_ip, bias, (uint32_t)n_cur, (int)B);
+    // group the batch's (neighbour r, pair p) back-links by r, p ascending within each r (counting sort, stable)
+    ANNB_CUDA(cudaMemcpyAsync(hsel.data(), dsel, (size_t)B * k * 8, cudaMemcpyDeviceToHost, h->stream));
+    ANNB_CUDA(cudaMemcpyAsync(hfound.data(), dfound, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
+    ANNB_CUDA(cudaStreamSynchronize(h->stream));
+    std::fill(cnt.begin(), cnt.begin() + n_cur, 0u);
+    for (int64_t i = 0; i < B; i++)
+      for (int j = 0; j < std::min(hfound[i], k); j++) {
+        const uint64_t r = hsel[(size_t)i * k + j];
+        if (r >= (uint64_t)n_cur) ANNB_FAIL(ANNB_ESTATE, "internal: GPU build selected node %llu of %lld", (unsigned long long)r, (long long)n_cur);
+        cnt[r]++;
+      }
+    hrows.clear();
+    hoff.clear();
+    uint32_t acc = 0;
+    for (int64_t r = 0; r < n_cur; r++)
+      if (cnt[r]) {
+        hrows.push_back((uint32_t)r);
+        hoff.push_back(acc);
+        pos[r] = acc;
+        acc += cnt[r];
+      }
+    hoff.push_back(acc);
+    hpairs.resize(acc);
+    for (int64_t i = 0; i < B; i++)
+      for (int j = 0; j < std::min(hfound[i], k); j++) hpairs[pos[hsel[(size_t)i * k + j]]++] = (uint32_t)(i * k + j);
+    const int R = (int)hrows.size();
+    ANNB_CUDA(cudaMemcpyAsync(dcsr, hoff.data(), hoff.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    ANNB_CUDA(cudaMemcpyAsync(dcsr + R + 1, hrows.data(), hrows.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    ANNB_CUDA(cudaMemcpyAsync(dcsr + 2 * R + 1, hpairs.data(), hpairs.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    if (R > 0)
+      reverse_link_kernel<<<(unsigned)((R + wb - 1) / wb), wb * 32, 0, h->stream>>>(b, dcsr + R + 1, dcsr, dcsr + 2 * R + 1, R, dseld, k, dq, dim,
+                                                                                    h->d_codebook, h->ds, is_ip, bias, (uint32_t)n_cur);
     h->launches += 2;
     ANNB_CUDA(cudaGetLastError());
     ANNB_CUDA(cudaStreamSynchronize(h->stream));  // hq / hlab are refilled next

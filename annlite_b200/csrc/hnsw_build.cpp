@@ -783,9 +783,9 @@ struct Worker {
 // Default insertion thread count (num_threads <= 0; the reference takes hardware_concurrency(),
 // hnsw_bindings.cpp:239-240).  The CPUs this process may actually run on are the smaller of the
 // affinity mask and the cgroup CPU quota -- a container that reports 128 logical CPUs but is
-// throttled to a fraction of them turns every held node lock into a convoy.  Capped at 32: on the
-// 2 x 64-thread hosts of the B200 boxes the 1M-point build took 27 s with 32 threads, 34 s with
-// 64 and 56 s with 128 (DESIGN.md section 5); callers that know better pass num_threads.
+// throttled to a fraction of them turns every held node lock into a convoy.  Capped at 32: more
+// threads than that made the 1M-point build slower, not faster, on 128-thread hosts (lock convoys);
+// callers that know better pass num_threads.
 int hnsw_default_threads() {
   int n = (int)std::thread::hardware_concurrency();
   if (n < 1) n = 1;

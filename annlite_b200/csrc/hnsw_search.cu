@@ -1,4 +1,4 @@
-// hnsw_search.cu -- K3: warp-per-query HNSW walk over PQ codes (sm_100a).
+// hnsw_search.cu -- K3: warp-per-query HNSW walk over PQ codes (sm_90a).
 //
 // Reference semantics: HierarchicalNSW::searchKnn (include/hnswlib/hnswalg.h:1237-1295) =
 // greedy descent on levels maxlevel..1 (:1248-1274) + searchBaseLayerST (:243-329), and the

@@ -17,7 +17,7 @@ _NO_TABLES = 'Row index exceeds or batch distance table uninitialized, most like
 def default_threads():
     """Insertion threads when the caller names none.  The reference takes hardware_concurrency()
     (hnsw_bindings.cpp:104); here, like ``hnsw_default_threads()`` in the library, the CPUs this process may really
-    use (affinity mask, cgroup quota), capped at 32 -- the measured optimum on the B200 hosts (DESIGN.md section 5)."""
+    use (affinity mask, cgroup quota), capped at 32 -- more threads than that contend on the node locks."""
     n = os.cpu_count() or 1
     try:
         n = min(n, len(os.sched_getaffinity(0)))

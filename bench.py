@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py -- queries/sec of the PQ-HNSW search path (BASELINE.json configs[1]: 1M x 128d fp32,
-M=8 PQ, HNSW M=16 ef_construction=200, ef=64, k=10) on N B200s of one node.
+M=8 PQ, HNSW M=16 ef_construction=200, ef=64, k=10) on N H100s of one node.
 
 A "step" is one pass of the hot path (ADC tables -> HNSW walk -> top-k; since round 2 ONE kernel, hnsw_walk4,
 which builds each query's table in shared memory) over one batch of synthetic queries.  Prints ONE JSON line (rank 0):
@@ -8,8 +8,13 @@ which builds each query's table in shared memory) over one batch of synthetic qu
   e2e       : same metric through the host-buffer C-ABI call (H2D of queries + K1 + K3 + D2H of results)
   roofline  : dominant kernel (K3 walk): algorithmic bytes / CUDA-event time vs measured HBM peak
   cpu_baseline : the C oracle port timed on the host cores on a bounded sample of the same batch
-`--impl reference` times the reference's own CPU path (oracle/_ref: compiled from /root/reference)
+`--impl reference` times the reference's own CPU path (oracle/_ref, compiled by oracle/build_ref.py)
 on the same config: batched get_dist_mat + knn_query with all host threads.
+`--dump-outputs DIR` writes what the headline (streamed, device-buffer) path returned in its last timed step as
+DIR/labels.npy (float64) and DIR/dists.npy (float32).  The inputs are seeded, the codebook is trained on one thread
+and the index builder is deterministic, so the same arguments give the same outputs on every run and two builds can be
+compared.  The index and the codebook are cached in a temporary directory (keyed by configuration and library
+build), never in the tree.
 
 Multi-GPU (`torchrun ... bench.py --gpus N`): the index is replicated (1M x 384 B records = 384 MB
 fits every GPU) and every rank serves its own query batch -> no data-path collective, weak
@@ -20,11 +25,13 @@ merge kernel.  With N > 1 the default run ALSO times that sharded step and repor
 not speed, at a size that fits one GPU -- configs[2] / configs[4] are the sizes it exists for).
 """
 import argparse
+import atexit
 import hashlib
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -32,7 +39,8 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-CACHE = os.path.join(ROOT, '.index_cache')
+CACHE = os.path.join(tempfile.gettempdir(), f'annlite_b200_bench_{os.getuid()}')   # the tree may be read-only
+H100_HBM_GBS = 3350.0   # NVIDIA data sheet, H100 SXM (HBM3): the roofline's bandwidth bound unless MEASURED_PEAKS.json says otherwise
 
 
 def filtered_leg(timeout_s=240):
@@ -84,6 +92,8 @@ def parse(argv=None):
     ap.add_argument('--pool', type=int, default=4, help='distinct query batches cycled through the steps')
     ap.add_argument('--no-filtered-leg', action='store_true',
                     help='skip the configs[3] side measurement (filtered search, child process, ~20 s, untimed)')
+    ap.add_argument('--dump-outputs', metavar='DIR',
+                    help='write the labels and distances of the last timed step to DIR/labels.npy and DIR/dists.npy')
     return ap.parse_args(argv)
 
 
@@ -120,8 +130,18 @@ def make_queries(a, nb, rank=0):
     return (centers[lab] + rng.standard_normal((nb, a.batch, a.dim), dtype=np.float32)).astype(np.float32)
 
 
+def _lib_tag():
+    """Digest of the built library: a cached index is reused only by the build that made it."""
+    from annlite_b200 import _lib
+    try:
+        with open(_lib.LIB_PATH, 'rb') as f:
+            return hashlib.md5(f.read()).hexdigest()[:12]
+    except OSError:
+        return 'nolib'
+
+
 def cfg_key(a, extra=''):
-    s = f'{a.n}-{a.dim}-{a.m}-{a.ks}-{a.M}-{a.efc}-{a.dist}-{a.metric}-{extra}'
+    s = f'{a.n}-{a.dim}-{a.m}-{a.ks}-{a.M}-{a.efc}-{a.dist}-{a.metric}-{extra}-{_lib_tag()}'
     return hashlib.md5(s.encode()).hexdigest()[:12]
 
 
@@ -133,19 +153,32 @@ def train_codebook(a, X10k):
     if os.path.exists(p) and not a.no_cache:
         return np.load(p)
     from sklearn.cluster import KMeans
+    from threadpoolctl import threadpool_limits
     ds = a.dim // a.m
     if a.metric == 'cosine':
         X10k = X10k / np.maximum(np.linalg.norm(X10k, axis=1, keepdims=True), 1e-12)
     cb = np.empty((a.m, a.ks, ds), dtype=np.float32)
-    for m in range(a.m):
-        km = KMeans(n_clusters=a.ks, max_iter=20, n_init=1, random_state=0).fit(X10k[:, m * ds:(m + 1) * ds])
-        cb[m] = km.cluster_centers_
+    with threadpool_limits(1):   # threaded k-means adds per-thread partial sums in a varying order: not reproducible
+        for m in range(a.m):
+            km = KMeans(n_clusters=a.ks, max_iter=20, n_init=1, random_state=0).fit(X10k[:, m * ds:(m + 1) * ds])
+            cb[m] = km.cluster_centers_
     np.save(p, cb)
     return cb
 
 
+def gpu_identity(gpu=0):
+    """Name and power limit of the card the numbers were measured on (read-only nvidia-smi query)."""
+    try:
+        out = subprocess.run(['nvidia-smi', f'--id={gpu}', '--query-gpu=name,power.limit,clocks.max.sm',
+                              '--format=csv,noheader,nounits'], capture_output=True, text=True, timeout=30).stdout
+        name, plim, mhz = [c.strip() for c in out.strip().splitlines()[0].split(',')]
+        return {'name': name, 'power_limit_w': float(plim), 'sm_max_mhz': float(mhz)}
+    except Exception as ex:
+        return {'unavailable': repr(ex)[:200]}
+
+
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled every 20 ms during the timed region (read-only queries)."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -158,6 +191,7 @@ class ClockSampler:
             self.p = subprocess.Popen(['nvidia-smi', f'--id={self.gpu}', f'--query-gpu={self.Q}',
                                        '--format=csv,noheader,nounits', '-lms', '20'],
                                       stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self._end)   # never outlive the benchmark, even when it fails before stop()
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
         except Exception:
@@ -167,31 +201,22 @@ class ClockSampler:
         for line in self.p.stdout:
             self.rows.append([c.strip() for c in line.split(',')])
 
+    def _end(self):
+        if self.p and self.p.poll() is None:
+            self.p.terminate()
+            self.p.wait()
+
     def stop(self):
         if not self.p:
             return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['unavailable']}
         time.sleep(0.15)
-        self.p.terminate()
+        self._end()
         sm = [float(r[1]) for r in self.rows if len(r) >= 8 and r[1].replace('.', '').isdigit()]
         mx = [float(r[2]) for r in self.rows if len(r) >= 8 and r[2].replace('.', '').isdigit()]
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
         reasons = [n for i, n in enumerate(names) if any(len(r) >= 8 and r[4 + i].lower().startswith('active') for r in self.rows)]
         return {'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': max(mx) if mx else None,
                 'reasons': reasons, 'samples': len(sm)}
-
-
-def ncu_traffic_bytes():
-    """DRAM bytes per K3 launch from the committed ncu capture of this same command (profiles/)."""
-    p = os.path.join(ROOT, 'profiles', 'r02_k3_walk4_fused_ncu.txt')
-    try:
-        tot = 0.0
-        for line in open(p):
-            f = line.split()
-            if f and f[0] in ('dram__bytes_read.sum', 'dram__bytes_write.sum'):
-                tot += float(f[1]) * {'Mbyte': 1e6, 'Gbyte': 1e9, 'Kbyte': 1e3, 'byte': 1}[f[2]]
-        return tot or None
-    except Exception:
-        return None
 
 
 def recall_at_k(pred, truth):
@@ -326,6 +351,8 @@ def run_ours(a):
         dist.init_process_group('nccl', device_id=torch.device('cuda', local))
     ncores = os.cpu_count() or 1
     shard_main = a.mode == 'shard' and world > 1
+    props = torch.cuda.get_device_properties(local)
+    gpu = dict(gpu_identity(local), sms=props.multi_processor_count)
 
     # ---- index: replicated on every rank (rank 0 builds, the others load the file) -----------------
     cb = train_codebook(a, make_base(a, 0, 10_000)) if rank == 0 else None
@@ -394,6 +421,11 @@ def run_ours(a):
         clocks.start()
         time.sleep(0.05)
     ms, launches = _timed(torch, dist, e, world, step_dev_stream, a.steps, a.warmup, drain)
+    if a.dump_outputs and rank == 0:
+        last = (a.warmup + a.steps - 1) & 1                         # the buffer pair the last timed step wrote
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        np.save(os.path.join(a.dump_outputs, 'labels.npy'), out_l2[last].cpu().numpy().astype(np.float64))
+        np.save(os.path.join(a.dump_outputs, 'dists.npy'), out_d2[last].cpu().numpy().astype(np.float32))
     ms_e2e, _ = _timed(torch, dist, e, world, step_e2e_stream, a.steps, max(3, a.warmup // 2), drain)
     ms_sync, _ = _timed(torch, dist, e, world, step_dev, a.steps, 3)            # one blocking call per step, for reference
     ms_e2e_sync, _ = _timed(torch, dist, e, world, step_e2e, a.steps, 3)
@@ -437,14 +469,11 @@ def run_ours(a):
             peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
         except Exception:
             pass
-        peak = float(peaks.get('hbm_gbs', 6650.0))
+        peak = float(peaks.get('hbm_gbs', H100_HBM_GBS))
         achieved = alg_bytes_launch / (kern_ms / 1e3) / 1e9
-        traffic = ncu_traffic_bytes() if (a.n == 1_000_000 and a.batch == 10_000) else None
         roof = {'bound': 'hbm', 'kernel': 'hnsw_walk4 (ADC table build fused into the walk)', 'achieved': round(achieved, 2),
-                'peak': peak, 'peak_source': 'MEASURED_PEAKS.json' if 'hbm_gbs' in peaks else 'fallback 6.65 TB/s',
-                'unit': 'GB/s', 'frac': round(achieved / peak, 5), 'traffic': traffic,
-                'traffic_source': 'committed profile profiles/r02_k3_walk4_fused_ncu.txt (ncu --set full of this workload): '
-                                  'dram__bytes_read.sum + dram__bytes_write.sum per launch; not re-measured in this run',
+                'peak': peak, 'peak_source': 'MEASURED_PEAKS.json' if 'hbm_gbs' in peaks else 'H100 SXM data sheet (3.35 TB/s)',
+                'unit': 'GB/s', 'frac': round(achieved / peak, 5),
                 'alg_bytes_per_launch': round(alg_bytes_launch),
                 'ms_per_launch': round(kern_ms, 4), 'alg_bytes_per_query': round(float(alg_bytes_q.mean()), 1),
                 'hops_per_query': round(float(hops.mean()), 2), 'nbrs_per_query': round(float(nbrs.mean()), 1),
@@ -471,8 +500,9 @@ def run_ours(a):
             e.scan_topk(tables=tbl, k=k)
             k2_ms_old = e.last_kernel_ms()['scan_ms']
             e.set_option('scan_kernel', 0)
-            if k2_ms and k2_ms > 0:
-                peak_lk = 148 * 32 * (ck['sm_mhz'] or 1965.0) * 1e6 if isinstance(ck, dict) else 148 * 32 * 1.965e9
+            mhz = (ck or {}).get('sm_mhz') or gpu.get('sm_max_mhz')
+            if k2_ms and k2_ms > 0 and mhz:
+                peak_lk = props.multi_processor_count * 32 * mhz * 1e6
                 lk = float(sample) * n * a.m
                 k2 = {'kernel': 'scan_topk_tiled2_kernel (16-query interleaved table tile, lanes = queries) + merge_topk_kernel',
                       'round1_kernel_ms': round(k2_ms_old, 3), 'ids_equal_round1_kernel': bool(np.array_equal(gt_i, gt_old)),
@@ -500,8 +530,8 @@ def run_ours(a):
             'config': {'workload': f'configs[1]: {a.n}x{a.dim} fp32 {a.dist}, PQ M={a.m} Ks={a.ks}, HNSW M={a.M} '
                                    f'efc={a.efc}, ef={a.ef}, k={a.k}, batch={a.batch} queries/step/GPU',
                        'parallelism': 'replicate' + str(world),
-                       'l2_policy': 'index (384 MB walk records) exceeds the 126 MB L2; query batches rotate '
-                                    f'through a pool of {nb}',
+                       'l2_policy': f'index ({n * g["size_data_per_element"] / 1e6:.0f} MB of level-0 records) against the '
+                                    f'{props.L2_cache_size / 2**20:.0f} MB L2; query batches rotate through a pool of {nb}',
                        'metric_space': a.metric, 'index_build_s': round(t_build, 1), 'host_cores': ncores,
                        'api': 'streamed: annb_search_submit/wait with two batches in flight (value and e2e); '
                               'blocking_call_value = one annb_search call at a time'},
@@ -511,7 +541,7 @@ def run_ours(a):
                     'blocking_call_value': round(total_q / (ms_e2e_sync / 1e3), 1),
                     'blocking_call_pageable_buffers_value': round(B * n_pg * world / (ms_e2e_pg / 1e3), 1)},
             'blocking_call_value': round(total_q / (ms_sync / 1e3), 1),
-            'gpu_launches': int(launches), 'clocks': ck, 'roofline': roof, 'cpu_baseline': cpu,
+            'gpu': gpu, 'gpu_launches': int(launches), 'clocks': ck, 'roofline': roof, 'cpu_baseline': cpu,
             'recall_at_k': {'vs_exhaustive_adc': rec_adc, 'vs_true_l2': rec_l2, 'sample': sample},
             'parity': parity, 'k2_exhaustive_scan': k2,
         }
@@ -585,7 +615,7 @@ def run_reference(a):
         return
     from oracle import ref_driver as R
     if not R.available():
-        print(json.dumps({'impl': 'reference', 'unavailable': 'oracle/_ref not built (needs /root/reference at build time)'}))
+        print(json.dumps({'impl': 'reference', 'unavailable': 'oracle/_ref not built (needs the reference sources at build time)'}))
         return
     ncores = os.cpu_count() or 1
     world = int(os.environ.get('WORLD_SIZE', 1))

@@ -1,5 +1,5 @@
 /*
- * annb.h -- C ABI of libannlite_b200.so: the B200 (sm_100a) implementation of AnnLite's
+ * annb.h -- C ABI of libannlite_b200.so: the H100 (sm_90a) implementation of AnnLite's
  * PQ-ADC / PQ-HNSW search path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  Every entry point below replaces one

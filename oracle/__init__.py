@@ -8,8 +8,8 @@ algorithm, wrapped with ctypes.  Only ``tests/``, ``__graft_entry__.smoke()`` an
 Besides the restatement, ``pq_oracle.c`` carries two functions that are NOT the reference's algorithm and
 say so: ``orc_single_list_walk`` / ``orc_flagged_walk``, scalar models of the product's visited-free walks.
 CPU tests run them beside the restatement to check the equivalence argument the CUDA kernels rest on (and
-which rows an exact fp32 tie may change); they are pinned to the kernel by a capture taken on a B200
-(``tests/test_b200_capture.py``).  Nothing measured or shipped goes through them.
+which rows an exact fp32 tie may change); they are pinned to the kernel by a stored capture of its output
+(``tests/test_walk_capture.py``, which also replays it on the GPU).  Nothing measured or shipped goes through them.
 
 Parity status: PINNED against outputs of the reference itself (compiled by
 ``oracle/build_ref.py`` into ``oracle/_ref``): see ``tests/test_oracle_vs_ref.py`` and the

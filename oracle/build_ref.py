@@ -12,7 +12,7 @@ files land in ``oracle/_ref/`` (git-ignored, but shipped to the GPU box by ``gpu
 
 Flags follow ``setup.py:125-151`` (``-O3 -fopenmp -std=c++14`` => ISO mode => no FMA
 contraction) except ``-march=native`` -> ``-march=x86-64-v3``: the artefact is built in a
-CPU-only container and executed on a different host (the B200 box); the PQ path is scalar
+CPU-only container and executed on a different host (the GPU host); the PQ path is scalar
 table look-ups, so the ISA level only guards against SIGILL, it does not change results.
 
 One build-time edit is applied to a *temporary* copy of ``hnsw_bindings.cpp``

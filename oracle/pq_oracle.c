@@ -380,8 +380,8 @@ ORC_API void orc_encode(const float *x, const float *cb, int64_t N, int M, int K
  * annlite_b200/csrc/hnsw_search.cu -- one sorted list of at most ef (distance, node, expanded) entries,
  * no visited set, no candidate heap, arrival order among equal keys).  CPU tests run it beside
  * orc_hnsw_search to check the equivalence argument of DESIGN.md section 4 at sizes where a Python model
- * is too slow, including which rows an exact fp32 tie may change.  Measured against the B200: on the
- * dumps of scripts/repro_shapes.py it reproduces the kernel's result sets and hop counts row for row.
+ * is too slow, including which rows an exact fp32 tie may change.  Pinned to the kernel by the capture in
+ * tests/golden/b200_capture_c5_ef256.npz: it reproduces the kernel's result sets and hop counts row for row.
  * Same arguments as orc_hnsw_search without filter; rows come back ascending by (dist, label).        */
 ORC_API int orc_single_list_walk(const uint8_t *level0, uint64_t size_per_elem, uint64_t offset_data,
                                  uint64_t label_offset, const uint8_t *links, const uint64_t *link_off,

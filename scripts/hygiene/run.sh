@@ -5,7 +5,7 @@
 set -euo pipefail
 ROOT="$(cd "$(dirname "$0")/../.." && pwd)"
 H="$ROOT/annlite_b200/csrc"; LIB="$ROOT/annlite_b200/lib/libannlite_b200.so"
-O="$(mktemp -d)"; NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"; ARCH="-gencode arch=compute_100a,code=sm_100a"
+O="$(mktemp -d)"; NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"; ARCH="-gencode arch=compute_90a,code=sm_90a"
 for f in adc_table adc_scan hnsw_search walk_fused walk_flagged4 gpu_build capi; do
   $NVCC $ARCH -O1 -g -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -c "$H/$f.cu" -o "$O/$f.o" &
 done

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """BASELINE.json configs[2] / configs[4] on G GPUs of one node (torchrun, one process per GPU):
 
-  configs[2]  10M x 768d, PQ M=32 + HNSW ef=128, k=100, range-sharded across 8 x B200, NCCL top-k merge
+  configs[2]  10M x 768d, PQ M=32 + HNSW ef=128, k=100, range-sharded across 8 x H100, NCCL top-k merge
   configs[4]  100M x 96d, PQ M=16, range-sharded, batch 4096, ef sweep 16 -> 256: QPS vs recall at 1/2/4/8 GPUs
 
 Every rank generates ITS slice of the base vectors (seeded, reproducible), encodes and builds its shard graph

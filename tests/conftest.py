@@ -13,7 +13,7 @@ CASES = ['l2_m4', 'cos_m8', 'ties_k16', 'ip_u16']
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
 
 
 def has_gpu():

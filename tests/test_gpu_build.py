@@ -1,8 +1,8 @@
 """GPU: batched insertion with the level-0 work on the device (gpu_build.cu; SURVEY.md section 8f rank 2, second
 half; reference addPoint include/hnswlib/hnswalg.h:1108-1235 with its PQ-mode neighbour rule).
 
-The graph is not the one a sequential build makes (neither is the reference's multi-threaded build), so what is
-checked is what the path needs: the host graph assembled from the device records is structurally sound
+The graph is not the one a sequential build makes (neither is the reference's multi-threaded build), but the same rows
+always give the same graph, whatever the thread count.  Otherwise what is checked is what the path needs: the host graph assembled from the device records is structurally sound
 (annb_set_graph re-validates every count / link / level), it IS the graph the GPU searches (oracle parity over it),
 every label is stored exactly once, recall@10 against the exhaustive ADC scan is on a par with the reference's sequential build of
 the same data (scripts/gpu_build_quality.py: equal within the +-0.05 scatter of threaded host builds), and the index keeps working as a normal one afterwards (host insertions, save / load)."""
@@ -86,6 +86,16 @@ def test_gpu_built_graph_is_sound_searchable_and_as_good_as_the_host_built_one(N
     l1, d1 = eg.search(tables=t, k=10, ef=64)
     l2, d2 = e2.search(tables=t, k=10, ef=64)
     assert np.array_equal(l1, l2) and np.array_equal(bits(d1), bits(d2))
+
+
+def test_gpu_build_is_deterministic_whatever_the_thread_count():
+    X = blobs(60_000, 64, 11)
+    rng = np.random.default_rng(3)
+    cb = np.stack([X[rng.choice(len(X), 256, replace=False), m * 8:(m + 1) * 8] for m in range(8)]).astype(np.float32)
+    a, b = build(X, cb, 8, 'euclidean', gpu=True, threads=-1).get_graph(), build(X, cb, 8, 'euclidean', gpu=True, threads=7).get_graph()
+    for key in ('data_level0', 'link_lists', 'element_levels'):
+        assert np.array_equal(np.asarray(a[key]), np.asarray(b[key])), key
+    assert a['enterpoint_node'] == b['enterpoint_node'] and a['max_level'] == b['max_level']
 
 
 def test_small_batches_and_existing_labels_take_the_host_path():

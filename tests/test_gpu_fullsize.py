@@ -9,7 +9,7 @@ C2  1M x 128d gaussian (bench.py's data), PQ M=8, HNSW M=16 efc=200, ef=64, k=10
 C4  1M x 128d cosine with a 50 % filter (benchmarks/filtering_bench.py shape): 2 000 queries against the oracle's
     searchKnnWithFilter restatement over the same graph: recall of ids >= 0.995, distances <= 1e-4 relative
     (the device l2_normalize differs from numpy's einsum in the last ulp; BASELINE.json's tolerance).
-About 3 minutes on the B200 hosts, almost all of it host-side index construction.
+A few minutes, almost all of it host-side index construction.
 """
 import os
 import sys
@@ -78,8 +78,8 @@ def test_c2_full_size_rows_identical_to_the_reference():
           f'hops/query {st[:, 0].mean():.2f}')
     clean = ties == 0
     # a walk that met no exact fp32 tie leaves no freedom at all; one that did hangs, in the reference, on
-    # std::priority_queue's heap order: rows may then differ in tie order and -- about 1 walk in 10^4 on this data
-    # (profiles/r01_tie_hunt.txt) -- in one expansion more or fewer
+    # std::priority_queue's heap order: rows may then differ in tie order and -- rarely, about 1 walk in 10^4 on
+    # this data -- in one expansion more or fewer
     assert (v[clean] == 'exact').all(), int((v[clean] != 'exact').sum())
     assert (v != 'exact').sum() <= n_tie_walks
     assert (v == 'diff').sum() <= 2
