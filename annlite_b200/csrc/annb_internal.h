@@ -123,7 +123,6 @@ struct SearchParams {
   int is_ip;            // IP / COSINE table form: bias - <cb, q>
   float bias;           // fp32(1/Ks), or 0 for the raw pq_bind form
   int out_internal;     // hnsw_walk4: write internal node ids instead of labels into out_labels (the GPU builder)
-  int prefetch;         // hnsw_walk4 L2 prefetch: bit 0 = the nearest unexpanded entry at hop start, bit 1 = candidates closer than it
   float *dump_tables;   // debug: (B, M, Ks) device buffer that receives the tables the walk used, or nullptr
   int64_t B;
   int k, ef;
@@ -225,7 +224,6 @@ struct annb_index {
   int64_t opt_walk_kernel = 0;     // plain search: 0 = hnsw_walk4 with fused K1 (default), 1 = round-1 kernels (K1 +
                                    // hnsw_walk_fast), 2 = hnsw_walk4 over materialised tables (K1 + TMA staging)
   int64_t opt_scan_kernel = 0;     // K2 scan + top-k: 0 = query-tiled kernel where it applies, 1 = round-1 kernel, 2 = tiled even for small inputs (tests), 3 = first tiled version, forced
-  int64_t opt_prefetch = 1;        // hnsw_walk4 record L2 prefetch (bit mask, see SearchParams::prefetch)
   int64_t opt_gpu_build = 1;       // add_items with num_threads != 1 and >= 16384 fresh rows: level-0 insertion on the GPU
   int64_t opt_gpu_build_frac = 16; // a GPU-built batch is at most 1/frac of the graph it is inserted into
   int64_t reserve_nodes = 0;       // sync_device_graph sizes the device graph for this many nodes (GPU builder)

@@ -1576,7 +1576,6 @@ int annb_set_option(annb_index_t *h, const char *name, int64_t value) {
   else if (!strcmp(name, "scan_kernel")) h->opt_scan_kernel = value;
   else if (!strcmp(name, "walk_kernel")) h->opt_walk_kernel = value;
   else if (!strcmp(name, "dump_tables")) h->opt_dump_tables = value;
-  else if (!strcmp(name, "prefetch")) h->opt_prefetch = value;
   else if (!strcmp(name, "gpu_build")) h->opt_gpu_build = value;
   else if (!strcmp(name, "gpu_build_frac")) h->opt_gpu_build_frac = value;
   else if (!strcmp(name, "reset_counters")) h->flagged_fallbacks = h->flagged_fallback_queries = 0;

@@ -32,10 +32,3 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         : "memory");
   } while (!ok);
 }
-// L2 prefetch of one 128-byte line (no register, no scoreboard): used to warm the record of a likely next node
-__device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-// The same through the TMA unit: ONE instruction of ONE lane pulls a whole record (bytes % 16 == 0, 16-byte aligned)
-// into L2 -- an asynchronous bulk copy with no destination but the cache (cp.async.bulk.prefetch.L2)
-__device__ __forceinline__ void bulk_prefetch_l2(const void *p, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}

@@ -203,7 +203,6 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       if (e2key != KEY_MAX) {
         const int e2src = __ffs(__ballot_sync(FULL_MASK, lm == e2key)) - 1;
         e2id = __shfl_sync(FULL_MASK, lv, e2src);  // (an unexpanded entry's value is its node id: no flag bit set)
-        if ((p.prefetch & 1) && lane * 128u < rec0_bytes) prefetch_l2(g.rec0 + (size_t)e2id * rec0_bytes + lane * 128u);
       }
       // expand that entry: ids are unique in the lists and an unexpanded entry's value IS its id
       auto take_e2 = [&]() {
@@ -373,7 +372,6 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
 template <int M, int EP, int EN>
 int launch_walk4f_t(annb_index *h, const SearchParams &p_in) {
   SearchParams p = p_in;
-  p.prefetch = (int)h->opt_prefetch;
   static_assert(w4f_fits(M, EP, EN, true) && w4f_fits(M, EP, EN, false), "walk4f geometry exceeds the SM's shared memory");
   auto kern = hnsw_walk4f<M, EP, EN>;
   const bool fused = p.queries != nullptr;

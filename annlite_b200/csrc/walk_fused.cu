@@ -174,9 +174,10 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
     // The two record register sets alternate roles (no copy, so nothing waits on a load before it is needed).
     auto hop = [&](Rec<M> &cur, Rec<M> &nxt) -> bool {
       hops++;
-      // ---- nearest not-yet-expanded list entry == candidate_set.top() (:268).  It is the next node unless this
-      // hop finds something closer, so its record is pulled into L2 FIRST: the DRAM round trip then overlaps the
-      // whole hop, and a wrong guess still leaves the record in L2 for the hop that does expand it ----
+      // ---- nearest not-yet-expanded list entry == candidate_set.top() (:268): the next node unless this hop finds
+      // something closer.  Nothing here may delay the scoring below: an L2 prefetch of this entry's record (or of
+      // the one after it) would stall the in-order issue until the reduction chain that finds it has resolved,
+      // and cost more than the record's lead gains (DESIGN §7) ----
       uint32_t lm = KEY_MAX;
 #pragma unroll
       for (int e = 0; e < EPL; e++) lm = min(lm, K[e] | (uint32_t)((int32_t)V[e] >> 31));
@@ -190,13 +191,6 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
         for (int e = EPL - 1; e >= 0; e--)
           if ((K[e] | (uint32_t)((int32_t)V[e] >> 31)) == e2key) myid = V[e] & IDM;  // lowest matching slot wins
         e2id = __shfl_sync(FULL_MASK, myid, e2src);
-        // (an L2 prefetch, not a register load: a second load into the same registers would have to wait for
-        // this one to land whenever a new candidate wins)
-        if (p.prefetch & 4) {         // bulk form: the TMA unit fetches the whole record on one lane's request
-          if (lane0) bulk_prefetch_l2(g.rec0 + (size_t)e2id * rec0_bytes, rec0_bytes);
-        } else if ((p.prefetch & 1) && lane * 128u < rec0_bytes) {
-          prefetch_l2(g.rec0 + (size_t)e2id * rec0_bytes + lane * 128u);
-        }
       }
       // expand that entry: flag it (the lowest matching slot of lane e2src)
       auto take_e2 = [&]() {
@@ -219,11 +213,6 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
         const int nv = __popc(__ballot_sync(FULL_MASK, valid));
         nbrs += nv;
         evals += nv;
-      }
-      if ((p.prefetch & 2) && mykey < e2key) {
-        // closer than everything still unexpanded: (one of) the next node(s) -- warm its record in L2 now
-        const uint8_t *rp = g.rec0 + (size_t)cur.link * rec0_bytes;
-        for (uint32_t o = 0; o < rec0_bytes; o += 128) prefetch_l2(rp + o);
       }
 
       // re-encounter of a listed node?  (an id can only be listed under this very key)
@@ -346,7 +335,6 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
 template <int M, int EPL>
 int launch_walk4_t(annb_index *h, const SearchParams &p_in) {
   SearchParams p = p_in;
-  p.prefetch = (int)h->opt_prefetch;
   static_assert(w4_fits(M, EPL, true) && w4_fits(M, EPL, false), "walk4 geometry exceeds the SM's shared memory");
   auto kern = hnsw_walk4<M, EPL>;
   const bool fused = p.queries != nullptr;

@@ -269,8 +269,8 @@ ANNB_API int annb_sync_counts(annb_index_t *h, int64_t *full_syncs, int64_t *pat
  * (filter / deletions: 0 hnsw_walk4f where it applies, 1 hnsw_walk_flagged), "flagged_en" (force hnsw_walk4f's
  * traversed-only list to 32 x value entries), "flagged_epl" (force hnsw_walk_flagged with 32 x value entries),
  * "force_general" (1 = filtered route without a filter, 2 = bitmap walk), "scan_kernel" (K2: 0 query-tiled where it
- * applies, 1 round-1 kernel, 2 tiled even for small inputs, 3 first tiled version), "prefetch", "warps_per_cta",
- * "ctas_per_sm", "gpu_build", "gpu_build_frac", "timing", "ip_raw", "dump_tables", "reset_counters". */
+ * applies, 1 round-1 kernel, 2 tiled even for small inputs, 3 first tiled version), "warps_per_cta", "ctas_per_sm",
+ * "gpu_build", "gpu_build_frac", "timing", "ip_raw", "dump_tables", "reset_counters". */
 ANNB_API int annb_set_option(annb_index_t *h, const char *name, int64_t value);
 
 #ifdef __cplusplus

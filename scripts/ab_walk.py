@@ -16,7 +16,6 @@ def main():
     ap.add_argument('--base-n', dest='n', type=int, default=1_000_000)
     ap.add_argument('--batch', type=int, default=10_000)
     ap.add_argument('--ef', type=int, default=64)
-    ap.add_argument('--prefetch', type=int, default=1)
     ap.add_argument('--short', action='store_true', help='few steps, no timing loop: for use under ncu')
     x = ap.parse_args()
     a = Bn.parse([])
@@ -26,7 +25,6 @@ def main():
     cb = Bn.train_codebook(a, Bn.make_base(a, 0, 10_000))
     e = Engine(a.dim, a.m, a.ks, a.metric, device=0)
     e.set_codebook(cb)
-    e.set_option('prefetch', x.prefetch)
     os.makedirs(Bn.CACHE, exist_ok=True)
     path = os.path.join(Bn.CACHE, f'ours_{Bn.cfg_key(a)}.hnsw')
     if os.path.exists(path):
