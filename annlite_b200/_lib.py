@@ -16,6 +16,12 @@ OK, EINVAL, ENODEVICE, ECUDA, ENOMEM, ESTATE, EFEWRESULTS, EIO, ECAPACITY, ENOTF
 HOST, DEVICE = 0, 1
 METRIC_L2, METRIC_IP, METRIC_COSINE = 0, 1, 2
 MAX_EF = 512
+ATTR_INTEGER, ATTR_FLOAT, ATTR_TEXT = 0, 1, 2
+MAX_ATTR_COLUMNS, FILTER_MAX_OPS, FILTER_MAX_DEPTH, FILTER_MAX_CONST_BYTES = 64, 256, 32, 32768
+(FOP_FALSE, FOP_TRUE, FOP_NOTNULL, FOP_INT_RANGE, FOP_INT_NE, FOP_INT_IN, FOP_INT_NIN, FOP_FLT_RANGE, FOP_FLT_NE,
+ FOP_FLT_IN, FOP_FLT_NIN, FOP_CODE_IN, FOP_AND, FOP_OR) = range(14)
+# annb_filter_op_t
+FILTER_OP = np.dtype([('op', '<i4'), ('col', '<i4'), ('a', '<i4'), ('b', '<i4')])
 
 _lib = None
 
@@ -59,6 +65,15 @@ PROTOTYPES = {
     'annb_search_submit': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _vp, _vp, _int, C.POINTER(_int)]),
     'annb_search_submit_filtered': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _vp, _int, _i64, _vp, _vp, _int, C.POINTER(_int)]),
     'annb_search_wait': (_int, [_vp, _int]),
+    'annb_attr_define': (_int, [_vp, _int, _int]),
+    'annb_attr_set': (_int, [_vp, _int, _vp, _i64, _vp, _vp, _int]),
+    'annb_attr_export': (_int, [_vp, _int, _vp, _vp, _i64, C.POINTER(_i64)]),
+    'annb_attr_clear': (_int, [_vp]),
+    'annb_filter_prepare': (_int, [_vp, _vp, _int, _vp, _i64, C.POINTER(_int), C.POINTER(_i64)]),
+    'annb_filter_labels': (_int, [_vp, _int, _vp, _i64, C.POINTER(_i64)]),
+    'annb_filter_release': (_int, [_vp, _int]),
+    'annb_search_prepared': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _int, _vp, _vp, _int]),
+    'annb_search_submit_prepared': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _int, _vp, _vp, _int, C.POINTER(_int)]),
     'annb_merge_topk': (_int, [_vp, _vp, _vp, _int, _i64, _int, _vp, _vp]),
     'annb_merge_topk_packed': (_int, [_vp, _vp, _int, _i64, _int, _i64, _i64, _vp, _vp, _int]),
     'annb_lane_stream': (_int, [_vp, _int, C.POINTER(_u64)]),

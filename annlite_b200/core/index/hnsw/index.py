@@ -14,8 +14,35 @@ from typing import List, Optional, Union
 
 import numpy as np
 
+from ....attributes import AttributeStore
 from ....enums import ExpandMode, Metric
 from ....hnsw_bind import Index
+
+
+class PreparedFilter:
+    """An attribute filter evaluated on the GPU once (HnswIndex.prepare_filter) and reused for any number of
+    batches.  `count` = admitted rows; `labels()` = their labels in insertion order.  It goes stale when the graph,
+    the deletions or the attributes change: a search with it then raises, and prepare_filter makes a fresh one."""
+
+    def __init__(self, engine, filter_id, count):
+        self._e, self.id, self.count = engine, filter_id, int(count)
+        self._labels = None
+
+    def labels(self):
+        if self._labels is None:
+            self._labels = self._e.filter_labels(self.id, self.count)
+        return self._labels
+
+    def release(self):
+        if self._e is not None and getattr(self._e, '_h', None) is not None and self._e._h.value:
+            self._e.filter_release(self.id)
+        self._e = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
 
 
 class HnswIndex:
@@ -23,7 +50,7 @@ class HnswIndex:
                  ef_search: int = 50, max_connection: int = 16, pq_codec=None,
                  index_file: Optional[Union[str, Path]] = None, initial_size: Optional[int] = None,
                  expand_step_size: int = 10240, expand_mode: ExpandMode = ExpandMode.STEP, device: int = 0,
-                 bruteforce_filter_below: Optional[int] = None, **kwargs):
+                 bruteforce_filter_below: Optional[int] = None, columns=None, **kwargs):
         assert expand_step_size > 0
         if isinstance(metric, str):
             metric = Metric.from_string(metric)
@@ -38,6 +65,8 @@ class HnswIndex:
         # opt-in: filters that admit at most this many ids are answered by an exact ADC scan over those ids
         # instead of the filtered graph walk (the reference's own TODO, hnsw/index.py:152); None = reference behaviour
         self.bruteforce_filter_below = bruteforce_filter_below
+        # attribute columns (annlite_b200.attributes): values by internal id in the library, filters on the GPU
+        self.attributes = AttributeStore(columns)
         if pq_codec is None:
             raise NotImplementedError('annlite_b200.HnswIndex is the PQ-encoded HNSW backend; pass a PQCodec '
                                       '(the float HNSW path is out of scope, SURVEY.md section 2 row 8)')
@@ -59,6 +88,9 @@ class HnswIndex:
             self._index.init_index(max_elements=self.capacity, ef_construction=self.ef_construction,
                                    M=self.max_connection, pq_codec=None)
         self._index.set_ef(self.ef_search)
+        self.attributes.reset_dictionaries()
+        if self._set_backend_pq:
+            self.attributes.attach(self._index._e)
 
     def _ensure_backend(self):
         if not self.pq_codec.is_trained:
@@ -66,6 +98,24 @@ class HnswIndex:
         if not self._set_backend_pq:
             self._index.loadPQ(self.pq_codec)
             self._set_backend_pq = True
+            self.attributes.attach(self._index._e)
+
+    # ---- attributes ---------------------------------------------------------------------------------
+    def set_attributes(self, ids, converted):
+        """Write tags converted by `attributes.convert` to the rows with these labels; every column is set."""
+        self._ensure_backend()
+        self.attributes.write(self._index._e, np.asarray(ids, dtype=np.uint64), converted)
+
+    def prepare_filter(self, where) -> PreparedFilter:
+        """Compile a filter dict (annlite_b200.filter) and evaluate it over every row on the GPU."""
+        self._ensure_backend()
+        program, consts = self.attributes.compile(where)
+        fid, count = self._index._e.filter_prepare(program, consts)
+        return PreparedFilter(self._index._e, fid, count)
+
+    def list_filter(self, prepared: PreparedFilter, order_by=None, ascending=True):
+        """The admitted labels in CellTable.query's order (annlite/storage/table.py:259-318)."""
+        return self.attributes.order(self._index._e, prepared.labels(), order_by, ascending)
 
     def load(self, index_file: Union[str, Path]):
         self._ensure_backend()
@@ -106,14 +156,19 @@ class HnswIndex:
         dists, ids = self.search_batch(self._prep(query)[:1], limit=limit, indices=indices)
         return dists[0], ids[0]
 
-    def search_batch(self, queries, limit: int = 10, indices=None, out_ids=None, out_dists=None):
+    def search_batch(self, queries, limit: int = 10, indices=None, out_ids=None, out_dists=None,
+                     filter: Optional[PreparedFilter] = None):
         """Batched search: (B, dim) -> (dists (B, limit), ids (B, limit)).  `queries` may be a numpy
-        array (host) or a torch CUDA tensor; device outputs can be supplied to stay on the GPU."""
+        array (host) or a torch CUDA tensor; device outputs can be supplied to stay on the GPU.  `filter` = a
+        PreparedFilter in place of `indices`: the same rules, its count standing in for len(indices)."""
         self._ensure_backend()
         if isinstance(queries, np.ndarray) or not hasattr(queries, 'data_ptr'):
             queries = self._prep(queries)
-        if indices is not None and len(indices) < limit:
-            limit = len(indices)
+        if filter is not None and indices is not None:
+            raise ValueError('pass either indices or a prepared filter')
+        n_allowed = filter.count if filter is not None else (len(indices) if indices is not None else None)
+        if n_allowed is not None and n_allowed < limit:
+            limit = n_allowed
         if limit <= 0:      # an empty candidate list: nothing can be returned (the reference would ask hnswlib for k=0)
             B = queries.shape[0]
             return np.empty((B, 0), dtype=np.float32), np.empty((B, 0), dtype=np.uint64)
@@ -122,12 +177,17 @@ class HnswIndex:
             raise ValueError(f'limit / ef_search above {MAX_EF} is not supported by the GPU walk (ANNB_MAX_EF); '
                              f'use PQIndex (exhaustive scan) or lower limit={limit} / ef_search={self.ef_search}')
         self._index.set_ef(max(self.ef_search, limit))
-        if (indices is not None and self.bruteforce_filter_below is not None
-                and len(indices) <= self.bruteforce_filter_below and out_ids is None):
-            ids, dists = self._index._e.scan_subset(queries, indices, k=limit, normalize=self._normalize_rounds)
+        if (n_allowed is not None and self.bruteforce_filter_below is not None
+                and n_allowed <= self.bruteforce_filter_below and out_ids is None):
+            subset = filter.labels() if filter is not None else indices
+            ids, dists = self._index._e.scan_subset(queries, subset, k=limit, normalize=self._normalize_rounds)
             return (np.sqrt(dists) if self.metric == Metric.EUCLIDEAN else dists), ids
-        ids, dists = self._index.knn_query_vectors(queries, k=limit, normalize=self._normalize_rounds,
-                                                   filters=indices, out_labels=out_ids, out_dists=out_dists)
+        if filter is not None:
+            ids, dists = self._index.knn_query_prepared(queries, filter.id, k=limit, normalize=self._normalize_rounds,
+                                                        out_labels=out_ids, out_dists=out_dists)
+        else:
+            ids, dists = self._index.knn_query_vectors(queries, k=limit, normalize=self._normalize_rounds,
+                                                       filters=indices, out_labels=out_ids, out_dists=out_dists)
         if self.metric == Metric.EUCLIDEAN:
             if isinstance(dists, np.ndarray):
                 dists = np.sqrt(dists)
@@ -135,20 +195,24 @@ class HnswIndex:
                 dists.sqrt_()
         return dists, ids
 
-    def search_batch_submit(self, queries, limit: int = 10, indices=None):
+    def search_batch_submit(self, queries, limit: int = 10, indices=None, filter: Optional[PreparedFilter] = None):
         """Streamed batched search for serving loops: returns a ticket at once, two batches can be in flight so
         the transfers (and the filter upload) of one overlap the graph walk of the other.  `indices` = the allowed
-        ids, as in `search` (hnsw/index.py:140-167)."""
+        ids, as in `search` (hnsw/index.py:140-167); `filter` = a PreparedFilter instead (nothing to upload)."""
         self._ensure_backend()
         if isinstance(queries, np.ndarray) or not hasattr(queries, 'data_ptr'):
             queries = self._prep(queries)
-        if indices is not None and len(indices) < limit:
+        if filter is not None and indices is not None:
+            raise ValueError('pass either indices or a prepared filter')
+        n_allowed = filter.count if filter is not None else (len(indices) if indices is not None else None)
+        if n_allowed is not None and n_allowed < limit:
             raise ValueError('fewer allowed ids than `limit`: use search_batch (it shrinks the limit like the reference)')
         from ...._lib import MAX_EF
         if max(self.ef_search, limit) > MAX_EF:
             raise ValueError(f'limit / ef_search above {MAX_EF} is not supported by the GPU walk (ANNB_MAX_EF)')
         self._index.set_ef(max(self.ef_search, limit))
-        return self._index.knn_query_submit(queries, k=limit, normalize=self._normalize_rounds, filters=indices)
+        return self._index.knn_query_submit(queries, k=limit, normalize=self._normalize_rounds, filters=indices,
+                                            prepared=filter.id if filter is not None else None)
 
     def search_batch_wait(self, ticket):
         ids, dists = self._index.knn_query_wait(ticket)

@@ -145,6 +145,35 @@ struct SearchParams {
 };
 
 // ------------------------------------------------------------------------------------------
+// attribute columns (annb_attr_*) and prepared filters (annb_filter_*)
+// ------------------------------------------------------------------------------------------
+struct AttrColumn {
+  int type = -1;                 // ANNB_ATTR_*, -1 = not declared
+  int width = 0;                 // bytes per value: 8 (INTEGER / FLOAT) or 4 (TEXT)
+  std::vector<uint8_t> vals;     // rows * width, by internal id (host: the source of truth)
+  std::vector<uint32_t> valid;   // validity bitmap by internal id
+  int64_t dirty_lo = 0, dirty_hi = 0;  // internal ids [lo, hi) not yet on the device
+  uint8_t *d_vals = nullptr;     // device copy
+  uint32_t *d_valid = nullptr;
+  size_t cap_vals = 0, cap_valid = 0;
+  int64_t dev_rows = 0;          // rows the device buffers hold
+};
+
+// what filter_eval_kernel reads for one column
+struct AttrColDev {
+  const void *vals;
+  const uint32_t *valid;
+  int32_t type;
+};
+
+struct PreparedFilter {
+  uint32_t *bits = nullptr;  // by-id bitmap, (n+31)/32 + 1 words: the layout of S_FLT_BY_ID
+  int64_t n = 0;             // rows it covers (gd.n at prepare time)
+  int64_t count = 0;         // admitted rows
+  uint64_t gen = 0;          // annb_index::state_gen at prepare time
+};
+
+// ------------------------------------------------------------------------------------------
 // the handle
 // ------------------------------------------------------------------------------------------
 struct annb_index {
@@ -228,6 +257,12 @@ struct annb_index {
   int64_t opt_gpu_build_frac = 16; // a GPU-built batch is at most 1/frac of the graph it is inserted into
   int64_t reserve_nodes = 0;       // sync_device_graph sizes the device graph for this many nodes (GPU builder)
   int64_t opt_dump_tables = 0;     // device pointer: searches copy the tables they used there (debug / parity tests)
+
+  // attribute columns and the filters prepared from them
+  std::vector<AttrColumn> attrs;
+  std::unordered_map<int, PreparedFilter> filters;
+  int next_filter_id = 1;
+  uint64_t state_gen = 1;          // bumped by every change to the graph, the deletions or the attributes
 };
 
 int annb_scratch(annb_index *h, int slot, size_t bytes, void **out);
@@ -244,7 +279,7 @@ enum {
   S_QUERIES = 0, S_TABLES, S_OUT_D, S_OUT_L, S_COUNTER, S_VISITED, S_TOUCHED, S_CAND,
   S_FOUND, S_STATS, S_FLT_LABELS, S_FLT_BY_LABEL, S_FLT_BY_ID, S_RAW0, S_CODES, S_MISC, S_PART_D, S_PART_I,
   S_L1_QUERIES, S_L1_TABLES, S_L1_OUT_D, S_L1_OUT_L, S_L1_FOUND, S_L0_FOUND, S_LANE_COUNTERS, S_QMAP,
-  S_L1_FLT_LABELS, S_L1_FLT_BY_LABEL, S_L1_FLT_BY_ID, S_SCRATCH_SLOTS
+  S_L1_FLT_LABELS, S_L1_FLT_BY_LABEL, S_L1_FLT_BY_ID, S_FILTER_PROG, S_FILTER_SCAN, S_FILTER_OUT, S_SCRATCH_SLOTS
 };
 static_assert(S_SCRATCH_SLOTS <= 32, "annb_index::d_scratch is too small");
 
@@ -272,6 +307,15 @@ int launch_merge_topk(annb_index *h, const uint64_t *labels, const float *dists,
                       int64_t d_gstride, uint64_t *labels_out, float *dists_out, cudaStream_t stream);
 int launch_filter_bitmap(annb_index *h, const uint64_t *d_filter_labels, int64_t n_filter, uint32_t *d_by_label,
                          uint32_t *d_by_id);
+// attr_filter.cu: evaluate a validated program over rows [0, n) into a by-id bitmap ((n+31)/32 + 1 words) and its
+// admitted count (device u64, accumulated: the caller zeroes it); compact a bitmap into the labels of its rows
+int launch_filter_eval(annb_index *h, const annb_filter_op_t *d_prog, int n_ops, const void *d_consts, int n_const_bytes,
+                       const AttrColDev *cols, int n_cols, int64_t n, const uint32_t *d_deleted, uint32_t *d_bits,
+                       unsigned long long *d_count);
+int launch_filter_compact(annb_index *h, const uint32_t *d_bits, int64_t n, const uint64_t *d_labels, uint64_t *d_out,
+                          unsigned int *d_block_scratch);
+// blocks launch_filter_compact uses for n rows (its scratch holds one u32 per block)
+int64_t filter_compact_blocks(int64_t n);
 
 // host builder
 int hnsw_insert_rows(annb_index *h, const uint8_t *codes, const uint64_t *labels, int64_t n, int num_threads,

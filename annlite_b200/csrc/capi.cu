@@ -79,6 +79,28 @@ int annb_pinned(annb_index *h, int slot, size_t bytes, void **out) {
     if (_rc) return _rc;     \
   } while (0)
 
+// ---- attribute rows follow the graph ----------------------------------------------------------------
+// size every column to the graph's capacity (new rows are NULL)
+static void attr_fit(annb_index *h) {
+  const int64_t rows = h->g.inited ? h->g.max_elements : 0;
+  for (AttrColumn &c : h->attrs) {
+    if (c.type < 0) continue;
+    if ((int64_t)c.vals.size() < rows * c.width) c.vals.resize((size_t)rows * c.width, 0);
+    if ((int64_t)c.valid.size() < (rows + 31) / 32 + 1) c.valid.resize((size_t)(rows + 31) / 32 + 1, 0u);
+  }
+}
+
+// the graph was replaced (init / load / adopted state): every row of every column is NULL again, schema kept
+static void graph_replaced(annb_index *h) {
+  h->state_gen++;
+  for (AttrColumn &c : h->attrs) {
+    std::fill(c.vals.begin(), c.vals.end(), 0);
+    std::fill(c.valid.begin(), c.valid.end(), 0u);
+    c.dirty_lo = 0;
+    c.dirty_hi = std::numeric_limits<int64_t>::max();
+  }
+}
+
 // stage an input: returns a device pointer (the caller's own if it already is one)
 static int stage_in(annb_index *h, const void *p, int space, size_t bytes, int slot, const void **out) {
   if (space == ANNB_DEVICE) {
@@ -169,6 +191,12 @@ int annb_destroy(annb_index_t *h) {
   if (h->d_up) cudaFree(h->d_up);
   if (h->d_labels) cudaFree(h->d_labels);
   if (h->d_deleted) cudaFree(h->d_deleted);
+  for (AttrColumn &c : h->attrs) {
+    if (c.d_vals) cudaFree(c.d_vals);
+    if (c.d_valid) cudaFree(c.d_valid);
+  }
+  for (auto &f : h->filters)
+    if (f.second.bits) cudaFree(f.second.bits);
   for (int i = 0; i < 6; i++)
     if (h->ev[i]) cudaEventDestroy(h->ev[i]);
   if (h->stream2) cudaStreamDestroy(h->stream2);
@@ -403,6 +431,7 @@ int annb_init_graph(annb_index_t *h, int64_t max_elements, int M, int ef_constru
   ANNB_ENTER(h);
   // M = 1 makes the level multiplier 1/ln(M) infinite (hnswalg.h:47) and the reference's level draw undefined
   if (max_elements < 0 || M < 2 || M > 1024) ANNB_FAIL(ANNB_EINVAL, "bad max_elements / M (2 <= M <= 1024)");
+  graph_replaced(h);
   ANNB_TRY(h->g.init(max_elements, M, ef_construction, random_seed, (size_t)h->M * h->code_bytes));
   h->dev_dirty = true;
   return ANNB_OK;
@@ -411,6 +440,7 @@ int annb_init_graph(annb_index_t *h, int64_t max_elements, int M, int ef_constru
 int annb_load_index(annb_index_t *h, const char *path, int64_t max_elements) {
   ANNB_ENTER(h);
   if (!path) ANNB_FAIL(ANNB_EINVAL, "null path");
+  graph_replaced(h);
   ANNB_TRY(h->g.load_file(path, max_elements, (size_t)h->M * h->code_bytes));
   h->dev_dirty = true;
   if (int rc = check_code_rows(h, h->g.level0 + h->g.offset_data, h->g.count.load(), h->g.size_per_elem)) {
@@ -440,6 +470,7 @@ int annb_set_graph(annb_index_t *h, const uint8_t *data_level0, uint64_t data_le
   HostGraph &g = h->g;
   const size_t crow = (size_t)h->M * h->code_bytes;
   if (max_elements < cur_element_count) max_elements = cur_element_count;
+  graph_replaced(h);
   ANNB_TRY(g.init(max_elements, M, ef_construction, 100, crow));
   if (g.size_per_elem != size_data_per_element) ANNB_FAIL(ANNB_EINVAL, "Invalid value of size_data_per_element_ ");
   if (g.label_offset != label_offset) ANNB_FAIL(ANNB_EINVAL, "Invalid value of label_offset_ ");
@@ -612,6 +643,7 @@ int annb_add_items(annb_index_t *h, const float *vectors, const void *codes, con
   if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
   if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised: call annb_init_graph first");
   if (n == 0) return ANNB_OK;
+  h->state_gen++;
   ANNB_CUDA(cudaStreamSynchronize(h->stream));   // insertion reuses search scratch: let streamed searches finish
   ANNB_CUDA(cudaStreamSynchronize(h->stream2));
   // num_threads == 1 is the reference's deterministic single-threaded build; any other value is an unordered
@@ -695,6 +727,7 @@ int annb_add_items_with_tables(annb_index_t *h, const void *codes, const float *
   if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised: call annb_init_graph first");
   if (n == 0) return ANNB_OK;
   ANNB_TRY(check_code_rows(h, (const uint8_t *)codes, n, (size_t)h->M * h->code_bytes));
+  h->state_gen++;
   HostTables t{tables, (size_t)h->M * h->Ks};
   int rc = hnsw_insert_rows(h, (const uint8_t *)codes, labels, n, num_threads, host_tables_next, &t, n);
   h->dev_dirty = true;
@@ -704,7 +737,10 @@ int annb_add_items_with_tables(annb_index_t *h, const void *codes, const float *
 int annb_resize_index(annb_index_t *h, int64_t new_max_elements) {
   ANNB_ENTER(h);
   if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
-  return h->g.resize(new_max_elements);
+  ANNB_TRY(h->g.resize(new_max_elements));
+  h->state_gen++;
+  attr_fit(h);
+  return ANNB_OK;
 }
 
 static int set_deleted(annb_index *h, uint64_t label, bool del) {
@@ -722,6 +758,7 @@ static int set_deleted(annb_index *h, uint64_t label, bool del) {
     g.num_deleted--;
   }
   h->deleted_dirty = true;
+  h->state_gen++;
   return ANNB_OK;
 }
 int annb_mark_deleted(annb_index_t *h, uint64_t label) {
@@ -983,11 +1020,28 @@ int sync_device_graph(annb_index *h) {
 extern "C" {
 
 // ---- K3 ---------------------------------------------------------------------------------------
+// The filter is either a label list (filter_labels, n_filter) or a prepared bitmap (pf, its count standing in for
+// n_filter); from there on both take the same route.
+static int search_impl(annb_index *h, const float *queries, const float *tables, int in_space, int64_t B, int normalize,
+                       int k, int ef, const uint64_t *filter_labels, int filter_space, int64_t n_filter,
+                       const PreparedFilter *pf, uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out);
+
 int annb_search(annb_index_t *h, const float *queries, const float *tables, int in_space, int64_t B, int normalize, int k,
                 int ef, const uint64_t *filter_labels, int filter_space, int64_t n_filter, uint64_t *labels_out,
                 float *dists_out, int out_space, int64_t *stats_out) {
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
+  return search_impl(h, queries, tables, in_space, B, normalize, k, ef, filter_labels, filter_space, n_filter, nullptr,
+                     labels_out, dists_out, out_space, stats_out);
+}
+
+}  // extern "C"
+
+static int search_impl(annb_index *h, const float *queries, const float *tables, int in_space, int64_t B, int normalize,
+                       int k, int ef, const uint64_t *filter_labels, int filter_space, int64_t n_filter,
+                       const PreparedFilter *pf, uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out) {
+  const bool has_filter = filter_labels || pf;
+  if (pf) n_filter = pf->count;
   ANNB_TRY(settle_flagged_lanes(h));
   if ((queries == nullptr) == (tables == nullptr)) ANNB_FAIL(ANNB_EINVAL, "exactly one of queries / tables must be given");
   if (B < 0 || k <= 0 || ef <= 0 || !labels_out || !dists_out) ANNB_FAIL(ANNB_EINVAL, "bad B/k/ef/outputs");
@@ -1017,7 +1071,7 @@ int annb_search(annb_index_t *h, const float *queries, const float *tables, int 
   // H2D of chunk c+1 overlaps the walk of chunk c, the walk of chunk c+1 fills the SMs that chunk c's
   // persistent launch leaves idle in its tail, and D2H of chunk c overlaps the walk of chunk c+1.
   {
-    const bool plain = !filter_labels && h->g.num_deleted == 0 && !h->opt_force_general;
+    const bool plain = !has_filter && h->g.num_deleted == 0 && !h->opt_force_general;
     int nch = (int)h->opt_chunks;
     if (nch == 0) nch = (B >= 32768) ? 4 : (B >= 4096 ? 2 : 1);
     if (nch > 8) nch = 8;
@@ -1086,9 +1140,9 @@ int annb_search(annb_index_t *h, const float *queries, const float *tables, int 
   // tables: handed in (the literal dtables argument), built inside the walk (plain search, hnsw_walk4), or by K1
   const size_t tbytes = (size_t)B * h->M * h->Ks * sizeof(float);
   const float *dt = nullptr, *dq_fused = nullptr;
-  const bool plain_search = !filter_labels && h->g.num_deleted == 0 && !h->opt_force_general;
+  const bool plain_search = !has_filter && h->g.num_deleted == 0 && !h->opt_force_general;
   // fraction of the nodes a filtered / deletion-aware walk can admit: sizes its lists
-  const double selectivity = filter_labels ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
+  const double selectivity = has_filter ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
                                            : 1.0 - (double)h->g.num_deleted / (double)std::max<int64_t>(1, h->gd.n);
   // the table is built inside the walk for the plain search (hnsw_walk4) and for the filtered one (hnsw_walk4f)
   const bool fuse_walk = walk4_can_fuse(h) && (plain_search || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, selectivity)));
@@ -1104,7 +1158,9 @@ int annb_search(annb_index_t *h, const float *queries, const float *tables, int 
   }
   // filter
   const uint32_t *dfilter = nullptr;
-  if (filter_labels) {
+  if (pf) {
+    dfilter = pf->bits;
+  } else if (filter_labels) {
     uint32_t *by_id;
     ANNB_TRY(annb_scratch(h, S_FLT_BY_ID, ((size_t)(h->gd.n + 31) / 32 + 1) * 4, (void **)&by_id));
     if (h->max_label > (uint64_t)h->gd.n * 64 + (1ull << 30)) {
@@ -1195,6 +1251,8 @@ int annb_search(annb_index_t *h, const float *queries, const float *tables, int 
       ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   return ANNB_OK;
 }
+
+extern "C" {
 
 int annb_scan_subset(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k,
                      const uint64_t *subset_labels, int64_t n_subset, uint64_t *labels_out, float *dists_out) {
@@ -1331,11 +1389,13 @@ static int lane_wait(annb_index *h, int lane) {
 }
 
 // one batch, enqueued entirely on one lane: H2D -> normalise -> [filter bitmap] -> walk (tables built inside) -> D2H
+// The filter is a label list or a prepared bitmap (pf), as in search_impl.
 static int submit_impl(annb_index *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
-                       const uint64_t *filter_labels, int filter_space, int64_t n_filter, uint64_t *labels_out, float *dists_out,
-                       int out_space, int *ticket_out) {
+                       const uint64_t *filter_labels, int filter_space, int64_t n_filter, const PreparedFilter *pf,
+                       uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
+  if (pf) n_filter = pf->count;
   if (!queries || !labels_out || !dists_out || !ticket_out || B <= 0 || k <= 0 || ef <= 0) ANNB_FAIL(ANNB_EINVAL, "bad arguments");
-  if (n_filter < 0 || (n_filter > 0 && !filter_labels)) ANNB_FAIL(ANNB_EINVAL, "bad filter");
+  if (n_filter < 0 || (n_filter > 0 && !filter_labels && !pf)) ANNB_FAIL(ANNB_EINVAL, "bad filter");
   if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
   if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
   if (h->opt_force_general == 2) ANNB_FAIL(ANNB_EINVAL, "streamed searches do not run on the bitmap walk: use annb_search");
@@ -1347,9 +1407,9 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   if (h->gd.n == 0) ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   const int ef_eff = std::max(ef, k);
   if (ef_eff > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, k)=%d exceeds ANNB_MAX_EF=%d", ef_eff, ANNB_MAX_EF);
-  const bool general = filter_labels != nullptr || h->g.num_deleted > 0 || h->opt_force_general;
-  const double selectivity = filter_labels ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
-                                           : 1.0 - (double)h->g.num_deleted / (double)std::max<int64_t>(1, h->gd.n);
+  const bool general = filter_labels != nullptr || pf || h->g.num_deleted > 0 || h->opt_force_general;
+  const double selectivity = (filter_labels || pf) ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
+                                                   : 1.0 - (double)h->g.num_deleted / (double)std::max<int64_t>(1, h->gd.n);
   const bool sparse_labels = h->max_label > (uint64_t)h->gd.n * 64 + (1ull << 30);
   const int ticket = (int)(h->next_ticket++ & 0x3fffffff);
   const int lane = ticket & 1;
@@ -1361,7 +1421,7 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   uint64_t *dl = labels_out;
   int32_t *dfound;
   unsigned int *counters;
-  uint32_t *by_id = nullptr, *by_label = nullptr;
+  uint32_t *by_id = pf ? pf->bits : nullptr, *by_label = nullptr;
   uint64_t *dflt = nullptr;
   // all scratch first: a (re)allocation synchronises both lanes, which is only safe before enqueuing
   if (host_in || normalize > 0)
@@ -1475,7 +1535,8 @@ int annb_search_submit(annb_index_t *h, const float *queries, int in_space, int6
                        uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
-  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, labels_out, dists_out, out_space, ticket_out);
+  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, nullptr, labels_out, dists_out, out_space,
+                     ticket_out);
 }
 
 int annb_search_submit_filtered(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
@@ -1484,8 +1545,8 @@ int annb_search_submit_filtered(annb_index_t *h, const float *queries, int in_sp
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
   if (!filter_labels && n_filter != 0) ANNB_FAIL(ANNB_EINVAL, "bad filter");
-  return submit_impl(h, queries, in_space, B, normalize, k, ef, filter_labels, filter_space, n_filter, labels_out, dists_out, out_space,
-                     ticket_out);
+  return submit_impl(h, queries, in_space, B, normalize, k, ef, filter_labels, filter_space, n_filter, nullptr, labels_out, dists_out,
+                     out_space, ticket_out);
 }
 
 int annb_search_wait(annb_index_t *h, int ticket) {
@@ -1581,6 +1642,302 @@ int annb_set_option(annb_index_t *h, const char *name, int64_t value) {
   else if (!strcmp(name, "reset_counters")) h->flagged_fallbacks = h->flagged_fallback_queries = 0;
   else ANNB_FAIL(ANNB_EINVAL, "unknown option %s", name);
   return ANNB_OK;
+}
+
+}  // extern "C"
+
+// ---- attribute columns and prepared filters ----------------------------------------------------------
+static int drain_lanes(annb_index *h) {  // streamed searches in flight finish before anything they read changes
+  if (h->device < 0) return ANNB_OK;
+  ANNB_TRY(settle_flagged_lanes(h));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream2));
+  return ANNB_OK;
+}
+
+static int attr_width(int type) { return type == ANNB_ATTR_TEXT ? 4 : 8; }
+
+// structural checks of a filter program; nothing runs before it passes
+static int validate_program(const annb_index *h, const annb_filter_op_t *prog, int n_ops, const void *consts,
+                            int64_t n_const_bytes) {
+  if (n_ops <= 0 || !prog) ANNB_FAIL(ANNB_EINVAL, "filter program is empty");
+  if (n_ops > ANNB_FILTER_MAX_OPS) ANNB_FAIL(ANNB_ELIMIT, "filter program has %d ops (limit %d)", n_ops, ANNB_FILTER_MAX_OPS);
+  if (n_const_bytes < 0 || (n_const_bytes > 0 && !consts) || n_const_bytes % 8)
+    ANNB_FAIL(ANNB_EINVAL, "filter constants: size must be a multiple of 8 bytes");
+  if (n_const_bytes > ANNB_FILTER_MAX_CONST_BYTES)
+    ANNB_FAIL(ANNB_ELIMIT, "filter constants take %lld bytes (limit %d)", (long long)n_const_bytes, ANNB_FILTER_MAX_CONST_BYTES);
+  int depth = 0;
+  for (int i = 0; i < n_ops; i++) {
+    const annb_filter_op_t &o = prog[i];
+    if (o.op < ANNB_FOP_FALSE || o.op > ANNB_FOP_OR) ANNB_FAIL(ANNB_EINVAL, "filter op %d: unknown op code %d", i, o.op);
+    if (o.op == ANNB_FOP_AND || o.op == ANNB_FOP_OR) {
+      if (depth < 2) ANNB_FAIL(ANNB_EINVAL, "filter op %d: AND / OR needs two operands", i);
+      depth--;
+      continue;
+    }
+    if (++depth > ANNB_FILTER_MAX_DEPTH) ANNB_FAIL(ANNB_ELIMIT, "filter program nests deeper than %d", ANNB_FILTER_MAX_DEPTH);
+    if (o.op == ANNB_FOP_FALSE || o.op == ANNB_FOP_TRUE) continue;
+    if (o.col < 0 || o.col >= (int)h->attrs.size() || h->attrs[o.col].type < 0)
+      ANNB_FAIL(ANNB_EINVAL, "filter op %d: no attribute column %d", i, o.col);
+    const int type = h->attrs[o.col].type;
+    int want = -1;
+    int64_t need = 0, align = 8;
+    switch (o.op) {
+      case ANNB_FOP_NOTNULL: want = type; break;
+      case ANNB_FOP_INT_RANGE: want = ANNB_ATTR_INTEGER; need = 16; break;
+      case ANNB_FOP_INT_NE: want = ANNB_ATTR_INTEGER; need = 8; break;
+      case ANNB_FOP_INT_IN: case ANNB_FOP_INT_NIN: want = ANNB_ATTR_INTEGER; need = 8 * (int64_t)o.b; break;
+      case ANNB_FOP_FLT_RANGE: want = ANNB_ATTR_FLOAT; need = 16; break;
+      case ANNB_FOP_FLT_NE: want = ANNB_ATTR_FLOAT; need = 8; break;
+      case ANNB_FOP_FLT_IN: case ANNB_FOP_FLT_NIN: want = ANNB_ATTR_FLOAT; need = 8 * (int64_t)o.b; break;
+      case ANNB_FOP_CODE_IN: want = ANNB_ATTR_TEXT; need = 4 * (((int64_t)o.b + 31) / 32); align = 4; break;
+    }
+    if (type != want) ANNB_FAIL(ANNB_EINVAL, "filter op %d: op %d does not apply to column %d of type %d", i, o.op, o.col, type);
+    if (o.b < 0) ANNB_FAIL(ANNB_EINVAL, "filter op %d: negative count", i);
+    if (o.op != ANNB_FOP_NOTNULL && (o.a < 0 || o.a % align || (int64_t)o.a + need > n_const_bytes))
+      ANNB_FAIL(ANNB_EINVAL, "filter op %d: constants [%d, %lld) outside the pool of %lld bytes or misaligned", i, o.a,
+                (long long)o.a + need, (long long)n_const_bytes);
+  }
+  if (depth != 1) ANNB_FAIL(ANNB_EINVAL, "filter program leaves %d values on the stack (must be 1)", depth);
+  return ANNB_OK;
+}
+
+// bring the device copy of a column up to date for rows [0, n): the dirty range, new rows, or all of it after a
+// reallocation
+static int attr_sync_dev(annb_index *h, AttrColumn &c, int64_t n) {
+  const size_t words = (size_t)(n + 31) / 32 + 1;
+  const size_t vbytes = (size_t)std::max<int64_t>(n, 1) * c.width;
+  int64_t lo = std::min(c.dirty_lo, c.dev_rows), hi = std::max(c.dirty_hi, n);
+  if (c.cap_vals < vbytes || c.cap_valid < words * 4 || !c.d_vals || !c.d_valid) {
+    ANNB_TRY(ensure_dev((void **)&c.d_vals, &c.cap_vals, vbytes));
+    ANNB_TRY(ensure_dev((void **)&c.d_valid, &c.cap_valid, words * 4));
+    lo = 0;
+  }
+  hi = std::min(hi, n);
+  if (hi > lo) {
+    ANNB_CUDA(cudaMemcpyAsync(c.d_vals + (size_t)lo * c.width, c.vals.data() + (size_t)lo * c.width, (size_t)(hi - lo) * c.width,
+                              cudaMemcpyHostToDevice, h->stream));
+  }
+  const size_t w0 = (size_t)std::max<int64_t>(lo, 0) / 32, w1 = words;  // validity: from the first dirty word to the end
+  if (w1 > w0)
+    ANNB_CUDA(cudaMemcpyAsync(c.d_valid + w0, c.valid.data() + w0, (w1 - w0) * 4, cudaMemcpyHostToDevice, h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));  // the host vectors may be written again as soon as this returns
+  c.dev_rows = n;
+  c.dirty_lo = std::numeric_limits<int64_t>::max();
+  c.dirty_hi = 0;
+  return ANNB_OK;
+}
+
+static int find_filter(annb_index *h, int filter_id, PreparedFilter **out) {
+  auto it = h->filters.find(filter_id);
+  if (it == h->filters.end()) ANNB_FAIL(ANNB_EINVAL, "no prepared filter %d", filter_id);
+  if (it->second.gen != h->state_gen)
+    ANNB_FAIL(ANNB_ESTATE, "prepared filter %d is stale: the graph, the deletions or the attributes changed since it was prepared",
+              filter_id);
+  *out = &it->second;
+  return ANNB_OK;
+}
+
+extern "C" {
+
+int annb_attr_define(annb_index_t *h, int col, int type) {
+  ANNB_ENTER(h);
+  if (type < ANNB_ATTR_INTEGER || type > ANNB_ATTR_TEXT) ANNB_FAIL(ANNB_EINVAL, "unknown attribute type %d", type);
+  if (col < 0 || col >= ANNB_MAX_ATTR_COLUMNS) ANNB_FAIL(ANNB_ELIMIT, "attribute column %d (limit %d columns)", col, ANNB_MAX_ATTR_COLUMNS);
+  if (col < (int)h->attrs.size()) {
+    if (h->attrs[col].type != type) ANNB_FAIL(ANNB_EINVAL, "attribute column %d is already declared with type %d", col, h->attrs[col].type);
+    return ANNB_OK;
+  }
+  if (col != (int)h->attrs.size()) ANNB_FAIL(ANNB_EINVAL, "attribute columns are declared in order: next is %d", (int)h->attrs.size());
+  h->attrs.emplace_back();
+  h->attrs.back().type = type;
+  h->attrs.back().width = attr_width(type);
+  h->attrs.back().dirty_lo = 0;
+  h->attrs.back().dirty_hi = std::numeric_limits<int64_t>::max();
+  attr_fit(h);
+  h->state_gen++;
+  return ANNB_OK;
+}
+
+int annb_attr_set(annb_index_t *h, int col, const uint64_t *labels, int64_t n, const void *values, const uint8_t *valid, int space) {
+  ANNB_ENTER(h);
+  if (col < 0 || col >= (int)h->attrs.size()) ANNB_FAIL(ANNB_EINVAL, "no attribute column %d", col);
+  if (n < 0 || (n > 0 && (!labels || !values))) ANNB_FAIL(ANNB_EINVAL, "null labels / values");
+  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
+  if (n == 0) return ANNB_OK;
+  AttrColumn &c = h->attrs[col];
+  std::vector<uint64_t> hl;
+  std::vector<uint8_t> hv, hvalid;
+  if (space == ANNB_DEVICE) {
+    ANNB_NEED_GPU(h);
+    hl.resize((size_t)n);
+    hv.resize((size_t)n * c.width);
+    ANNB_CUDA(cudaMemcpy(hl.data(), labels, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    ANNB_CUDA(cudaMemcpy(hv.data(), values, (size_t)n * c.width, cudaMemcpyDeviceToHost));
+    labels = hl.data();
+    values = hv.data();
+    if (valid) {
+      hvalid.resize((size_t)n);
+      ANNB_CUDA(cudaMemcpy(hvalid.data(), valid, (size_t)n, cudaMemcpyDeviceToHost));
+      valid = hvalid.data();
+    }
+  }
+  std::vector<uint32_t> ids((size_t)n);
+  for (int64_t i = 0; i < n; i++) {
+    auto it = h->g.label_lookup.find(labels[i]);
+    if (it == h->g.label_lookup.end()) ANNB_FAIL(ANNB_ENOTFOUND, "Label not found");
+    ids[i] = it->second;
+    if (c.type == ANNB_ATTR_TEXT && (!valid || valid[i])) {
+      int32_t code;
+      memcpy(&code, (const uint8_t *)values + (size_t)i * 4, 4);
+      if (code < 0) ANNB_FAIL(ANNB_EINVAL, "TEXT codes must be >= 0 (row %lld has %d)", (long long)i, code);
+    }
+  }
+  ANNB_TRY(drain_lanes(h));
+  attr_fit(h);
+  for (int64_t i = 0; i < n; i++) {
+    const uint32_t id = ids[i];
+    const bool ok = !valid || valid[i];
+    if (ok) memcpy(c.vals.data() + (size_t)id * c.width, (const uint8_t *)values + (size_t)i * c.width, (size_t)c.width);
+    else memset(c.vals.data() + (size_t)id * c.width, 0, (size_t)c.width);
+    if (ok) c.valid[id >> 5] |= 1u << (id & 31);
+    else c.valid[id >> 5] &= ~(1u << (id & 31));
+    c.dirty_lo = std::min<int64_t>(c.dirty_lo, id);
+    c.dirty_hi = std::max<int64_t>(c.dirty_hi, (int64_t)id + 1);
+  }
+  h->state_gen++;
+  return ANNB_OK;
+}
+
+int annb_attr_export(annb_index_t *h, int col, void *values, uint8_t *valid, int64_t cap, int64_t *n_out) {
+  ANNB_ENTER(h);
+  if (col < 0 || col >= (int)h->attrs.size()) ANNB_FAIL(ANNB_EINVAL, "no attribute column %d", col);
+  if (cap < 0) ANNB_FAIL(ANNB_EINVAL, "negative capacity");
+  attr_fit(h);
+  const AttrColumn &c = h->attrs[col];
+  const int64_t rows = h->g.inited ? h->g.count.load() : 0;
+  const int64_t m = std::min(cap, rows);
+  if (values && m) memcpy(values, c.vals.data(), (size_t)m * c.width);
+  if (valid)
+    for (int64_t i = 0; i < m; i++) valid[i] = (uint8_t)((c.valid[i >> 5] >> (i & 31)) & 1u);
+  if (n_out) *n_out = rows;
+  return ANNB_OK;
+}
+
+int annb_attr_clear(annb_index_t *h) {
+  ANNB_ENTER(h);
+  ANNB_TRY(drain_lanes(h));
+  for (AttrColumn &c : h->attrs) {
+    if (c.d_vals) cudaFree(c.d_vals);
+    if (c.d_valid) cudaFree(c.d_valid);
+  }
+  h->attrs.clear();
+  h->state_gen++;
+  return ANNB_OK;
+}
+
+int annb_filter_prepare(annb_index_t *h, const annb_filter_op_t *program, int n_ops, const void *consts, int64_t n_const_bytes,
+                        int *filter_id, int64_t *count) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  if (!filter_id || !count) ANNB_FAIL(ANNB_EINVAL, "null outputs");
+  *filter_id = 0;
+  *count = 0;
+  ANNB_TRY(validate_program(h, program, n_ops, consts, n_const_bytes));
+  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
+  ANNB_TRY(drain_lanes(h));
+  ANNB_TRY(sync_device_graph(h));
+  attr_fit(h);
+  const int64_t n = h->gd.n;
+  std::vector<AttrColDev> cols(h->attrs.size());
+  std::vector<char> used(h->attrs.size(), 0);
+  for (int i = 0; i < n_ops; i++)
+    if (program[i].op != ANNB_FOP_AND && program[i].op != ANNB_FOP_OR && program[i].op > ANNB_FOP_TRUE) used[program[i].col] = 1;
+  for (size_t c = 0; c < h->attrs.size(); c++) {
+    if (!used[c]) continue;
+    ANNB_TRY(attr_sync_dev(h, h->attrs[c], n));
+    cols[c] = AttrColDev{h->attrs[c].d_vals, h->attrs[c].d_valid, h->attrs[c].type};
+  }
+  const size_t words = (size_t)(n + 31) / 32 + 1;
+  const size_t pbytes = (size_t)n_ops * sizeof(annb_filter_op_t);
+  uint8_t *dprog;
+  ANNB_TRY(annb_scratch(h, S_FILTER_PROG, pbytes + (size_t)n_const_bytes + 16, (void **)&dprog));
+  unsigned long long *dcount = (unsigned long long *)(dprog + pbytes + n_const_bytes);  // both multiples of 8
+  PreparedFilter f;
+  f.n = n;
+  f.gen = h->state_gen;
+  ANNB_CUDA(cudaMalloc(&f.bits, words * 4));
+  int rc = ANNB_OK;
+  unsigned long long hcount = 0;
+  if (cudaMemcpyAsync(dprog, program, pbytes, cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+      (n_const_bytes && cudaMemcpyAsync(dprog + pbytes, consts, (size_t)n_const_bytes, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) ||
+      cudaMemsetAsync(dcount, 0, 8, h->stream) != cudaSuccess)
+    rc = ANNB_ECUDA;
+  if (rc == ANNB_OK)
+    rc = launch_filter_eval(h, (const annb_filter_op_t *)dprog, n_ops, dprog + pbytes, (int)n_const_bytes, cols.data(), (int)cols.size(),
+                            n, h->gd.deleted, f.bits, dcount);
+  if (rc == ANNB_OK && (cudaMemcpyAsync(&hcount, dcount, 8, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
+                        cudaStreamSynchronize(h->stream) != cudaSuccess))
+    rc = ANNB_ECUDA;
+  if (rc != ANNB_OK) {
+    cudaFree(f.bits);
+    if (rc == ANNB_ECUDA) annb_set_error("CUDA error while evaluating a filter: %s", cudaGetErrorString(cudaGetLastError()));
+    return rc;
+  }
+  f.count = (int64_t)hcount;
+  const int id = h->next_filter_id++;
+  h->filters[id] = f;
+  *filter_id = id;
+  *count = f.count;
+  return ANNB_OK;
+}
+
+int annb_filter_labels(annb_index_t *h, int filter_id, uint64_t *labels_out, int64_t cap, int64_t *n_out) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  if (cap < 0 || (cap > 0 && !labels_out)) ANNB_FAIL(ANNB_EINVAL, "bad output buffer");
+  PreparedFilter *f;
+  ANNB_TRY(find_filter(h, filter_id, &f));
+  if (n_out) *n_out = f->count;
+  const int64_t m = std::min(cap, f->count);
+  if (m == 0) return ANNB_OK;
+  unsigned int *dscan;
+  uint64_t *dout;
+  ANNB_TRY(annb_scratch(h, S_FILTER_SCAN, (size_t)filter_compact_blocks(f->n) * 4, (void **)&dscan));
+  ANNB_TRY(annb_scratch(h, S_FILTER_OUT, (size_t)f->count * 8, (void **)&dout));
+  ANNB_TRY(launch_filter_compact(h, f->bits, f->n, h->d_labels, dout, dscan));
+  ANNB_CUDA(cudaMemcpyAsync(labels_out, dout, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  return ANNB_OK;
+}
+
+int annb_filter_release(annb_index_t *h, int filter_id) {
+  ANNB_ENTER(h);
+  auto it = h->filters.find(filter_id);
+  if (it == h->filters.end()) ANNB_FAIL(ANNB_EINVAL, "no prepared filter %d", filter_id);
+  ANNB_TRY(drain_lanes(h));  // a streamed batch may still walk (or re-run on) this bitmap
+  if (it->second.bits) ANNB_CUDA(cudaFree(it->second.bits));
+  h->filters.erase(it);
+  return ANNB_OK;
+}
+
+int annb_search_prepared(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef, int filter_id,
+                         uint64_t *labels_out, float *dists_out, int out_space) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  PreparedFilter *f;
+  ANNB_TRY(find_filter(h, filter_id, &f));
+  return search_impl(h, queries, nullptr, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, f, labels_out, dists_out, out_space,
+                     nullptr);
+}
+
+int annb_search_submit_prepared(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
+                                int filter_id, uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  PreparedFilter *f;
+  ANNB_TRY(find_filter(h, filter_id, &f));
+  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, f, labels_out, dists_out, out_space, ticket_out);
 }
 
 }  // extern "C"

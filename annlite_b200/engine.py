@@ -281,6 +281,82 @@ class Engine:
         finally:
             getattr(self, '_inflight', {}).pop(ticket, None)
 
+    # ---- attribute columns and prepared filters -----------------------------------------------
+    _ATTR_DTYPE = {L.ATTR_INTEGER: np.int64, L.ATTR_FLOAT: np.float64, L.ATTR_TEXT: np.int32}
+
+    def attr_define(self, col, attr_type):
+        L.check(self._lib.annb_attr_define(self._h, int(col), int(attr_type)))
+
+    def attr_set(self, col, attr_type, labels, values, valid=None):
+        """Set column `col` of the rows with these labels; `valid` (bool per row) marks NULLs."""
+        lab = np.ascontiguousarray(labels, dtype=np.uint64)
+        val = np.ascontiguousarray(values, dtype=self._ATTR_DTYPE[attr_type])
+        assert lab.shape == val.shape and lab.ndim == 1
+        vp = None
+        if valid is not None:
+            valid = np.ascontiguousarray(valid, dtype=np.uint8)
+            assert valid.shape == lab.shape
+            vp = valid.ctypes.data
+        L.check(self._lib.annb_attr_set(self._h, int(col), lab.ctypes.data, lab.shape[0], val.ctypes.data, vp, L.HOST))
+
+    def attr_export(self, col, attr_type):
+        """(values, valid) of column `col` by internal id."""
+        n = self.element_count
+        vals = np.empty(max(n, 1), dtype=self._ATTR_DTYPE[attr_type])
+        valid = np.empty(max(n, 1), dtype=np.uint8)
+        got = C.c_int64()
+        L.check(self._lib.annb_attr_export(self._h, int(col), vals.ctypes.data, valid.ctypes.data, n, C.byref(got)))
+        return vals[:n], valid[:n].astype(bool)
+
+    def attr_clear(self):
+        L.check(self._lib.annb_attr_clear(self._h))
+
+    def filter_prepare(self, program, consts):
+        """program: FILTER_OP records, consts: bytes (a multiple of 8) -> (filter id, admitted count)."""
+        prog = np.ascontiguousarray(program, dtype=L.FILTER_OP)
+        cst = np.frombuffer(bytes(consts), dtype=np.uint8) if len(consts) else np.zeros(8, dtype=np.uint8)
+        fid, cnt = C.c_int(), C.c_int64()
+        L.check(self._lib.annb_filter_prepare(self._h, prog.ctypes.data if prog.size else None, int(prog.shape[0]),
+                                              cst.ctypes.data, len(consts), C.byref(fid), C.byref(cnt)))
+        return fid.value, cnt.value
+
+    def filter_labels(self, filter_id, count):
+        out = np.empty(max(int(count), 1), dtype=np.uint64)
+        n = C.c_int64()
+        L.check(self._lib.annb_filter_labels(self._h, int(filter_id), out.ctypes.data, int(count), C.byref(n)))
+        return out[:n.value]
+
+    def filter_release(self, filter_id):
+        L.check(self._lib.annb_filter_release(self._h, int(filter_id)))
+
+    def search_prepared(self, queries, filter_id, k=10, ef=50, normalize=0, out_labels=None, out_dists=None):
+        q = self._as_f32(queries)
+        B = q.shape[0]
+        if out_labels is None:
+            out_labels = np.empty((B, k), dtype=np.uint64)
+            out_dists = np.empty((B, k), dtype=np.float32)
+        qp, qs, _k0 = L.as_ptr(q)
+        lp, ls, _k1 = L.as_ptr(out_labels)
+        dp, ds_, _k2 = L.as_ptr(out_dists)
+        assert ls == ds_
+        L.check(self._lib.annb_search_prepared(self._h, qp, qs, B, int(normalize), int(k), int(ef), int(filter_id), lp, dp, ls))
+        return out_labels, out_dists
+
+    def search_submit_prepared(self, queries, filter_id, out_labels, out_dists, k=10, ef=50, normalize=0):
+        """Streamed form of search_prepared: a ticket for search_wait, as search_submit."""
+        q = self._as_f32(queries)
+        qp, qs, k0 = L.as_ptr(q)
+        lp, ls, k1 = L.as_ptr(out_labels)
+        dp, ds_, k2 = L.as_ptr(out_dists)
+        assert ls == ds_
+        t = C.c_int()
+        L.check(self._lib.annb_search_submit_prepared(self._h, qp, qs, q.shape[0], int(normalize), int(k), int(ef),
+                                                      int(filter_id), lp, dp, ls, C.byref(t)))
+        self._inflight = getattr(self, '_inflight', {})
+        self._inflight[t.value] = (k0, k1, k2, None)
+        self._next_ticket = t.value + 1
+        return t.value
+
     def merge_topk(self, labels_gbk, dists_gbk, out_labels, out_dists):
         G, B, k = labels_gbk.shape
         L.check(self._lib.annb_merge_topk(self._h, labels_gbk.data_ptr(), dists_gbk.data_ptr(), G, B, k,

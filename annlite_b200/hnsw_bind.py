@@ -202,10 +202,17 @@ class Index:
         return self._e.search(queries=queries, k=int(k), ef=self.default_ef, normalize=normalize,
                               filter_labels=filters, out_labels=out_labels, out_dists=out_dists)
 
-    def knn_query_submit(self, queries, k=1, normalize=0, out_labels=None, out_dists=None, filters=None):
+    def knn_query_prepared(self, queries, filter_id, k=1, normalize=0, out_labels=None, out_dists=None):
+        """Extension: knn_query_vectors under a prepared attribute filter (annb_search_prepared)."""
+        self._need_pq()
+        return self._e.search_prepared(queries, filter_id, k=int(k), ef=self.default_ef, normalize=normalize,
+                                       out_labels=out_labels, out_dists=out_dists)
+
+    def knn_query_submit(self, queries, k=1, normalize=0, out_labels=None, out_dists=None, filters=None, prepared=None):
         """Extension: streamed form of knn_query_vectors / knn_query_with_filter (annb_search_submit[_filtered]):
         returns a ticket; up to two batches are in flight.  `knn_query_wait(ticket)` returns (labels, dists).
-        `filters` = the allowed labels, as in knn_query_with_filter (hnsw_bindings.cpp:393-516)."""
+        `filters` = the allowed labels, as in knn_query_with_filter (hnsw_bindings.cpp:393-516); `prepared` = the id
+        of a prepared attribute filter instead (annb_search_submit_prepared)."""
         self._need_pq()
         B = queries.shape[0]
         if out_labels is None:
@@ -213,8 +220,12 @@ class Index:
             out_dists = np.empty((B, int(k)), dtype=np.float32)
         if filters is not None and (isinstance(filters, np.ndarray) or not hasattr(filters, 'data_ptr')):
             filters = np.ascontiguousarray(filters, dtype=np.uint64)
-        t = self._e.search_submit(queries, out_labels, out_dists, k=int(k), ef=self.default_ef, normalize=normalize,
-                                  filter_labels=filters)
+        if prepared is not None:
+            t = self._e.search_submit_prepared(queries, prepared, out_labels, out_dists, k=int(k), ef=self.default_ef,
+                                               normalize=normalize)
+        else:
+            t = self._e.search_submit(queries, out_labels, out_dists, k=int(k), ef=self.default_ef, normalize=normalize,
+                                      filter_labels=filters)
         self._tickets = getattr(self, '_tickets', {})
         self._tickets[t] = (out_labels, out_dists)
         return t

@@ -4,20 +4,25 @@ SQLite or RocksDB, which are out of scope: SURVEY.md section 2 rows 17-19).
 
 One cell (n_cells == 1), PQ required.  `index()` accepts an ndarray (ids = running offsets, which
 is what CellTable hands out, annlite/storage/table.py:213-257) or any object with `.embeddings`
-(+ optional `.ids`).  `search()` returns `(dists, ids)` arrays; a `filter` is given as the array of
-admissible ids (what CellTable.query would yield, container.py:107-120).
+(+ optional `.ids`).  `search()` returns `(dists, ids)` arrays; a `filter` is either the array of
+admissible ids (what CellTable.query would yield, container.py:107-120) or, with `columns=`, a filter
+dict (annlite/filter.py) that is compiled and evaluated on the GPU (annlite_b200.filter).
 """
 import datetime
 import hashlib
+import logging
 import shutil
 from pathlib import Path
 from typing import Optional, Union
 
 import numpy as np
 
+from .attributes import ATTRS_FILE, normalize_columns
 from .core.codec.pq import PQCodec
 from .core.index.hnsw.index import HnswIndex
 from .enums import Metric
+
+logger = logging.getLogger(__name__)
 
 
 class AnnLite:
@@ -26,7 +31,7 @@ class AnnLite:
                  n_components: Optional[int] = None, initial_size: Optional[int] = None,
                  expand_step_size: int = 10240, data_path: Union[Path, str] = Path('./data'),
                  create_if_missing: bool = True, read_only: bool = False, verbose: bool = False, device: int = 0,
-                 **kwargs):
+                 columns=None, filterable_attrs=None, **kwargs):
         if 'dim' in kwargs:
             n_dim = kwargs.pop('dim')
         if n_cells != 1:
@@ -48,7 +53,11 @@ class AnnLite:
         if self._pq_codec_path.exists():
             self._pq_codec = PQCodec.load(self._pq_codec_path)     # reads the reference's own pickles too
             self._pq_codec.device = device
-        self._kwargs = dict(initial_size=initial_size, expand_step_size=expand_step_size, device=device, **kwargs)
+        if columns is not None and filterable_attrs:
+            logger.warning('`filterable_attrs` will be overwritten by `columns`.')      # annlite/index.py:152-158
+        self.columns = normalize_columns(columns if columns is not None else filterable_attrs)
+        self._kwargs = dict(initial_size=initial_size, expand_step_size=expand_step_size, device=device,
+                            columns=self.columns, **kwargs)
         self._index = None
         self._n = 0
         if self._pq_codec.is_trained:
@@ -139,8 +148,20 @@ class AnnLite:
         ids = getattr(docs, 'ids', None)
         return x, (np.asarray(ids) if ids is not None else None)
 
-    def index(self, docs, ids=None, num_threads: int = -1, **kwargs):
-        """annlite/index.py:274-295 -> CellContainer.insert (container.py:262-308)."""
+    @staticmethod
+    def _doc_tags(docs, tags):
+        """The row attributes: `tags` as given (per-row dicts or column -> values), else the docs' own `.tags`."""
+        if tags is not None or isinstance(docs, np.ndarray):
+            return tags
+        try:
+            rows = [d.tags for d in docs]
+        except (TypeError, AttributeError):
+            return None
+        return rows
+
+    def index(self, docs, ids=None, num_threads: int = -1, tags=None, **kwargs):
+        """annlite/index.py:274-295 -> CellContainer.insert (container.py:262-308).  `tags` = the rows' attributes
+        (a list of dicts or a dict of column -> values); without it the docs' `.tags` are used when present."""
         if self.read_only:
             return
         if not self.is_trained:
@@ -150,7 +171,11 @@ class AnnLite:
         if ids is None:
             ids = doc_ids
         offsets = np.arange(self._n, self._n + n, dtype=np.int64) if ids is None else np.asarray(ids, dtype=np.int64)
+        tags = self._doc_tags(docs, tags)
+        attrs = self._index.attributes.convert(tags, n) if (self.columns and tags is not None) else None
         self._index.add_with_ids(x, offsets, num_threads=num_threads)
+        if attrs is not None:
+            self._index.set_attributes(offsets, attrs)
         # `_n` is the next implicit offset: past every label handed out OR handed in (a caller-supplied id range
         # must not be reused for later documents without ids: the graph would treat them as in-place updates)
         self._n = max(self._n + (n if ids is None else 0), int(offsets.max()) + 1 if n else 0)
@@ -159,15 +184,18 @@ class AnnLite:
     # ---- search ---------------------------------------------------------------------------------------
     def search_numpy(self, query_np: 'np.ndarray', filter=None, limit: int = 10, **kwargs):
         """annlite/index.py:485-522: (dists (B, limit), ids (B, limit)); EUCLIDEAN distances are sqrt'ed
-        like HnswIndex.search does."""
+        like HnswIndex.search does.  `filter` = a filter dict over the columns, or the admissible ids."""
         if not self.is_trained:
             raise RuntimeError('The indexer is not trained, cannot add new documents')
         self._sanity_check(query_np)
         indices = None
         if filter is not None and not (isinstance(filter, dict) and not filter):
             if isinstance(filter, dict):
-                raise NotImplementedError('attribute filters need the SQLite cell table (out of scope); '
-                                          'pass the admissible ids as an array instead')
+                prepared = self._index.prepare_filter(filter)
+                try:
+                    return self._index.search_batch(query_np, limit=limit, filter=prepared)
+                finally:
+                    prepared.release()
             indices = np.asarray(filter)
             if indices.dtype == bool:
                 indices = np.nonzero(indices)[0]
@@ -189,21 +217,42 @@ class AnnLite:
     def search_by_vectors(self, query_np, filter=None, limit: int = 10, **kwargs):
         return self.search_numpy(query_np, filter=filter, limit=limit)
 
-    def update(self, docs, ids=None, num_threads: int = -1, **kwargs):
+    def update(self, docs, ids=None, num_threads: int = -1, tags=None, **kwargs):
         """annlite/index.py:297-332 -> CellContainer.update (container.py:323-386): stored ids are re-added, which
-        the graph handles as an in-place update (hnswalg.h:1119-1131); unknown ids are inserted."""
+        the graph handles as an in-place update (hnswalg.h:1119-1131); unknown ids are inserted.  Given `tags` (or
+        docs with `.tags`), they replace the rows' attributes -- also for a row that stays where it is, which the
+        reference leaves with its old tags (container.py:342-347)."""
         x, doc_ids = self._embeddings(docs)
         if ids is None:
             ids = doc_ids
         if ids is None:
             raise ValueError('update needs the ids of the vectors')
-        self._sanity_check(x)
+        n, _ = self._sanity_check(x)
         ids = np.asarray(ids, dtype=np.int64)
+        tags = self._doc_tags(docs, tags)
+        attrs = self._index.attributes.convert(tags, n) if (self.columns and tags is not None) else None
         self._index.add_with_ids(x, ids, num_threads=num_threads)
+        if attrs is not None:
+            self._index.set_attributes(ids, attrs)
         self._n = max(self._n, int(ids.max()) + 1)
 
     def delete(self, ids, **kwargs):
         self._index.delete([int(i) for i in ids])
+
+    def filter(self, filter, limit: int = 10, offset: int = 0, order_by: Optional[str] = None, ascending: bool = True,
+               **kwargs):
+        """annlite/index.py:389-422 -> CellTable.query (table.py:259-318): the labels of the rows the filter admits,
+        in insertion order or by `order_by` (NULL lowest, ties in insertion order; `ascending=False` reverses all),
+        then `offset` rows skipped and at most `limit` returned (`limit <= 0`: all of them)."""
+        if not self.is_trained:
+            raise RuntimeError('The indexer is not trained, cannot add new documents')
+        prepared = self._index.prepare_filter(filter or {})
+        try:
+            rows = self._index.list_filter(prepared, order_by=order_by, ascending=ascending)
+        finally:
+            prepared.release()
+        offset = max(int(offset), 0)
+        return rows[offset:offset + limit] if limit > 0 else rows[offset:]
 
     def clear(self):
         """annlite/index.py:539-545 for the part kept here: an empty graph of the initial capacity."""
@@ -259,6 +308,8 @@ class AnnLite:
         target.mkdir(parents=True)
         try:
             self._index.dump(target / 'cell_0.hnsw')
+            if self.columns:     # only with columns: other workspaces keep the reference's exact layout
+                self._index.attributes.dump(self._index._index._e, target / ATTRS_FILE)
         except Exception:
             shutil.rmtree(target, ignore_errors=True)
             raise
@@ -274,6 +325,8 @@ class AnnLite:
         if snap is None:
             raise FileNotFoundError(f'no snapshot of parameter set {self.params_hash} under {self.data_path}')
         self._index.load(snap / 'cell_0.hnsw')
+        if self.columns and (snap / ATTRS_FILE).exists():
+            self._index.attributes.load(self._index._index._e, snap / ATTRS_FILE)
         # labels may be sparse (caller-supplied ids): implicit offsets continue past the largest one
         native = getattr(self._index, '_index', None)
         ids = native.get_ids_list() if (native is not None and self._index.size) else []

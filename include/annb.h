@@ -232,6 +232,86 @@ ANNB_API int annb_search_submit_filtered(annb_index_t *h, const float *queries, 
                                 uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out);
 ANNB_API int annb_search_wait(annb_index_t *h, int ticket);
 
+/* ---- attribute columns and prepared filters ---------------------------------------------------
+ * The attribute columns of CellTable (annlite/storage/table.py:160-257), kept by internal id next to the graph:
+ * INTEGER -> int64, FLOAT -> double, TEXT -> int32 dictionary code (the code <-> string dictionaries live with the
+ * caller).  Every column has a validity bitmap; a row that was never set is NULL.  The host store is the source of
+ * truth and follows the graph: it grows with annb_resize_index, new rows are NULL, and annb_init_graph /
+ * annb_load_index / annb_set_graph reset every row to NULL (the schema stays).  Its device copy is brought up to
+ * date by dirty range on the next annb_filter_prepare.
+ *
+ * A filter (the WHERE clause CellTable.query runs, annlite/filter.py:17-90) is given as a postfix program of
+ * annb_filter_op_t plus a constant pool.  Every leaf pushes one bool per row (NULL rows push false); AND / OR pop two
+ * and push one; the program must leave exactly one value.  annb_filter_prepare evaluates it over every row on the
+ * GPU, ANDs in "not deleted" and keeps the result as a by-id bitmap owned by the handle.  There is no CPU
+ * evaluator: on a host-only handle (device == -1) the store works but prepare and the searches return
+ * ANNB_ENODEVICE. */
+#define ANNB_ATTR_INTEGER 0 /* int64 values  */
+#define ANNB_ATTR_FLOAT 1   /* double values */
+#define ANNB_ATTR_TEXT 2    /* int32 dictionary codes (>= 0) */
+
+#define ANNB_MAX_ATTR_COLUMNS 64
+#define ANNB_FILTER_MAX_OPS 256
+#define ANNB_FILTER_MAX_DEPTH 32
+#define ANNB_FILTER_MAX_CONST_BYTES 32768 /* the program and its constants sit in shared memory */
+
+/* op codes.  `a` is a byte offset into the constant pool, `b` a count; numeric constants are 8-byte aligned. */
+#define ANNB_FOP_FALSE 0     /* push false                                                            */
+#define ANNB_FOP_TRUE 1      /* push true (NULL rows too)                                             */
+#define ANNB_FOP_NOTNULL 2   /* push "column col is not NULL"                                         */
+#define ANNB_FOP_INT_RANGE 3 /* INTEGER col: lo <= v <= hi, consts[a] = {int64 lo, int64 hi}         */
+#define ANNB_FOP_INT_NE 4    /* INTEGER col: v != c, consts[a] = int64 c                              */
+#define ANNB_FOP_INT_IN 5    /* INTEGER col: v in consts[a .. a + 8b), int64, sorted ascending         */
+#define ANNB_FOP_INT_NIN 6   /* INTEGER col: v not in that list                                       */
+#define ANNB_FOP_FLT_RANGE 7 /* FLOAT col: lo <= v <= hi, consts[a] = {double lo, double hi}          */
+#define ANNB_FOP_FLT_NE 8    /* FLOAT col: v != c                                                     */
+#define ANNB_FOP_FLT_IN 9    /* FLOAT col: v in consts[a .. a + 8b), double, sorted ascending          */
+#define ANNB_FOP_FLT_NIN 10  /* FLOAT col: v not in that list                                         */
+#define ANNB_FOP_CODE_IN 11  /* TEXT col: bit v of the u32 bitset consts[a ..] of b bits (v >= b: 0)  */
+#define ANNB_FOP_AND 12
+#define ANNB_FOP_OR 13
+
+typedef struct {
+  int32_t op;
+  int32_t col;
+  int32_t a;
+  int32_t b;
+} annb_filter_op_t;
+
+/* Declare column `col` (0 <= col < ANNB_MAX_ATTR_COLUMNS, in order) with type ANNB_ATTR_*.  Redeclaring a column
+ * with its own type is a no-op; with another type, ANNB_EINVAL. */
+ANNB_API int annb_attr_define(annb_index_t *h, int col, int type);
+/* Set column `col` of the rows with the given labels: values = n entries of the column's width (int64 / double /
+ * int32), valid = n bytes (0 = NULL) or NULL for all valid.  Host memory (space == ANNB_HOST) or device memory.
+ * Every label is checked first: an unknown one gives ANNB_ENOTFOUND and nothing is written.  Streamed searches
+ * in flight are drained first, as insertions do. */
+ANNB_API int annb_attr_set(annb_index_t *h, int col, const uint64_t *labels, int64_t n, const void *values,
+                  const uint8_t *valid, int space);
+/* Copy column `col` out by internal id (the order of annb_get_labels): values (cap entries of its width) and
+ * valid (cap bytes); *n_out = number of rows (the element count).  Either output may be NULL. */
+ANNB_API int annb_attr_export(annb_index_t *h, int col, void *values, uint8_t *valid, int64_t cap, int64_t *n_out);
+/* Drop every column (schema and values). */
+ANNB_API int annb_attr_clear(annb_index_t *h);
+/* Validate the program (op codes, columns and their types, constant ranges and alignment, stack balance and depth:
+ * ANNB_EINVAL, or ANNB_ELIMIT beyond the limits above) before anything runs, bring the device columns up to date,
+ * evaluate it into a bitmap the handle owns and return its id and the number of admitted rows.  One blocking call
+ * per filter.  Any later change to the graph, the deletions or the attributes makes the filter stale: using it
+ * then returns ANNB_ESTATE (prepare it again). */
+ANNB_API int annb_filter_prepare(annb_index_t *h, const annb_filter_op_t *program, int n_ops, const void *consts,
+                        int64_t n_const_bytes, int *filter_id, int64_t *count);
+/* The labels a prepared filter admits, in internal-id order (insertion order).  Writes min(cap, count) labels
+ * and sets *n_out = count. */
+ANNB_API int annb_filter_labels(annb_index_t *h, int filter_id, uint64_t *labels_out, int64_t cap, int64_t *n_out);
+ANNB_API int annb_filter_release(annb_index_t *h, int filter_id);
+/* annb_search and annb_search_submit_filtered with a prepared filter in place of the label list: the bitmap is the
+ * prepared one and the filter's size is its admitted count; everything else (kernel choice, list sizing, re-runs of
+ * overflowing queries, ANNB_EFEWRESULTS) is the filtered route of those calls. */
+ANNB_API int annb_search_prepared(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k,
+                         int ef, int filter_id, uint64_t *labels_out, float *dists_out, int out_space);
+ANNB_API int annb_search_submit_prepared(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize,
+                                int k, int ef, int filter_id, uint64_t *labels_out, float *dists_out, int out_space,
+                                int *ticket_out);
+
 /* ---- shard merge (CellContainer.ivf_search merge rule, annlite/container.py:130-138) ---------- */
 
 /* G per-shard result lists (G,B,k) (as all-gathered over NCCL) -> (B,k) global top-k by

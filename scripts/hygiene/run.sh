@@ -6,13 +6,13 @@ set -euo pipefail
 ROOT="$(cd "$(dirname "$0")/../.." && pwd)"
 H="$ROOT/annlite_b200/csrc"; LIB="$ROOT/annlite_b200/lib/libannlite_b200.so"
 O="$(mktemp -d)"; NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"; ARCH="-gencode arch=compute_90a,code=sm_90a"
-for f in adc_table adc_scan hnsw_search walk_fused walk_flagged4 gpu_build capi; do
+for f in adc_table adc_scan hnsw_search walk_fused walk_flagged4 gpu_build attr_filter capi; do
   $NVCC $ARCH -O1 -g -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -c "$H/$f.cu" -o "$O/$f.o" &
 done
 g++ -O1 -g -std=c++17 -fPIC -fvisibility=hidden -ffp-contract=off -march=x86-64-v3 -fsanitize=address,undefined -fno-omit-frame-pointer \
     -I/usr/local/cuda/include -c "$H/hnsw_build.cpp" -o "$O/hnsw_build.o" &
 wait
-$NVCC $ARCH -shared -o "$O/asan.so" "$O"/{adc_table,adc_scan,hnsw_search,walk_fused,walk_flagged4,gpu_build,capi,hnsw_build}.o -Xlinker --exclude-libs,ALL -lpthread -Xcompiler -fsanitize=address,-fsanitize=undefined
+$NVCC $ARCH -shared -o "$O/asan.so" "$O"/{adc_table,adc_scan,hnsw_search,walk_fused,walk_flagged4,gpu_build,attr_filter,capi,hnsw_build}.o -Xlinker --exclude-libs,ALL -lpthread -Xcompiler -fsanitize=address,-fsanitize=undefined
 cp "$LIB" "$O/good.so"; trap 'cp "$O/good.so" "$LIB"' EXIT
 cp "$O/asan.so" "$LIB"
 export LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)"
