@@ -18,6 +18,7 @@ METRIC_L2, METRIC_IP, METRIC_COSINE = 0, 1, 2
 MAX_EF = 512
 ATTR_INTEGER, ATTR_FLOAT, ATTR_TEXT = 0, 1, 2
 MAX_ATTR_COLUMNS, FILTER_MAX_OPS, FILTER_MAX_DEPTH, FILTER_MAX_CONST_BYTES = 64, 256, 32, 32768
+FILTER_MAX_PER_CALL, FILTER_LAUNCH_MAX_OPS, FILTER_LAUNCH_MAX_CONST_BYTES = 1024, 2048, 65536
 (FOP_FALSE, FOP_TRUE, FOP_NOTNULL, FOP_INT_RANGE, FOP_INT_NE, FOP_INT_IN, FOP_INT_NIN, FOP_FLT_RANGE, FOP_FLT_NE,
  FOP_FLT_IN, FOP_FLT_NIN, FOP_CODE_IN, FOP_AND, FOP_OR) = range(14)
 # annb_filter_op_t
@@ -74,7 +75,10 @@ PROTOTYPES = {
     'annb_filter_release': (_int, [_vp, _int]),
     'annb_search_prepared': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _int, _vp, _vp, _int]),
     'annb_search_submit_prepared': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _int, _vp, _vp, _int, C.POINTER(_int)]),
-    'annb_merge_topk': (_int, [_vp, _vp, _vp, _int, _i64, _int, _vp, _vp]),
+    'annb_filter_prepare_many': (_int, [_vp, _int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'annb_search_multi': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _vp, _vp, _vp, _int]),
+    'annb_search_submit_multi': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _vp, _vp, _vp, _int, C.POINTER(_int)]),
+    'annb_merge_topk': (_int,[_vp, _vp, _vp, _int, _i64, _int, _vp, _vp]),
     'annb_merge_topk_packed': (_int, [_vp, _vp, _int, _i64, _int, _i64, _i64, _vp, _vp, _int]),
     'annb_lane_stream': (_int, [_vp, _int, C.POINTER(_u64)]),
     'annb_last_kernel_ms': (_int, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float)]),

@@ -45,6 +45,62 @@ class PreparedFilter:
             pass
 
 
+class QueryFilters:
+    """One attribute filter per query of a batch (HnswIndex.prepare_filters), evaluated on the GPU in one call.
+    Queries whose filters compile to the same program share one bitmap.  `ids[i]` = the library's filter id of query i
+    (0 = no filter), `counts[i]` = the rows its filter admits (-1 = no filter).  It goes stale like PreparedFilter."""
+
+    def __init__(self, engine, ids, counts):
+        self._e = engine
+        self.ids = np.ascontiguousarray(ids, dtype=np.int32)
+        self.counts = np.ascontiguousarray(counts, dtype=np.int64)
+        self._labels = {}
+
+    def __len__(self):
+        return len(self.ids)
+
+    @property
+    def distinct(self):
+        """the distinct filter ids in first-use order"""
+        ids = self.ids[self.ids != 0]
+        _, first = np.unique(ids, return_index=True)
+        return ids[np.sort(first)]
+
+    def labels(self, filter_id):
+        if filter_id not in self._labels:
+            count = int(self.counts[np.flatnonzero(self.ids == filter_id)[0]])
+            self._labels[filter_id] = self._e.filter_labels(int(filter_id), count)
+        return self._labels[filter_id]
+
+    def release(self):
+        if self._e is not None and getattr(self._e, '_h', None) is not None and self._e._h.value:
+            for fid in self.distinct.tolist():
+                self._e.filter_release(int(fid))
+        self._e = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+
+def dedupe_compiled(compiled):
+    """[(program, consts) or None per query] -> (distinct list, index of each query's program in it or -1).  Two
+    filters are the same when the compiler made the same program and constants of them."""
+    distinct, where, index = [], {}, []
+    for c in compiled:
+        if c is None:
+            index.append(-1)
+            continue
+        key = (np.ascontiguousarray(c[0]).tobytes(), bytes(c[1]))
+        if key not in where:
+            where[key] = len(distinct)
+            distinct.append(c)
+        index.append(where[key])
+    return distinct, np.asarray(index, dtype=np.int64)
+
+
 class HnswIndex:
     def __init__(self, dim: int, dtype=np.float32, metric: Metric = Metric.COSINE, ef_construction: int = 200,
                  ef_search: int = 50, max_connection: int = 16, pq_codec=None,
@@ -113,6 +169,68 @@ class HnswIndex:
         fid, count = self._index._e.filter_prepare(program, consts)
         return PreparedFilter(self._index._e, fid, count)
 
+    def prepare_filters(self, filters) -> QueryFilters:
+        """One filter dict per query ({} or None = no filter) -> QueryFilters.  Each dict is compiled; dicts that
+        compile to the same program are evaluated once, and all distinct ones in one call on the GPU."""
+        self._ensure_backend()
+        compiled = [None if (f is None or (isinstance(f, dict) and not f)) else self.attributes.compile(f) for f in filters]
+        distinct, index = dedupe_compiled(compiled)
+        ids = np.zeros(len(compiled), dtype=np.int32)
+        counts = np.full(len(compiled), -1, dtype=np.int64)
+        if distinct:
+            fids, fcounts = self._index._e.filter_prepare_many(distinct)
+            has = index >= 0
+            ids[has], counts[has] = fids[index[has]], fcounts[index[has]]
+        return QueryFilters(self._index._e, ids, counts)
+
+    def _search_per_query(self, queries, limit, qf: QueryFilters, out_ids=None, out_dists=None):
+        """search_batch with one filter per query: rows grouped by their shrunk limit (and the brute-force route),
+        each group one call; rows whose filter admits fewer than `limit` rows are padded (UINT64_MAX, +inf)."""
+        B = queries.shape[0]
+        if len(qf) != B:
+            raise ValueError(f'{len(qf)} filters for {B} queries')
+        from ...._lib import MAX_EF
+        k_row = np.where(qf.counts < 0, limit, np.minimum(qf.counts, limit))
+        if max(self.ef_search, int(k_row.max(initial=0))) > MAX_EF:
+            raise ValueError(f'limit / ef_search above {MAX_EF} is not supported by the GPU walk (ANNB_MAX_EF); '
+                             f'use PQIndex (exhaustive scan) or lower limit={limit} / ef_search={self.ef_search}')
+        brute = np.zeros(B, dtype=bool)
+        if self.bruteforce_filter_below is not None and out_ids is None:
+            brute = (qf.counts >= 0) & (qf.counts <= self.bruteforce_filter_below)
+        if out_ids is not None:
+            if np.any(k_row != limit):
+                raise ValueError('device outputs need every filter to admit at least `limit` rows')
+            self._index.set_ef(max(self.ef_search, limit))
+            ids, dists = self._index.knn_query_multi(queries, qf.ids, k=limit, normalize=self._normalize_rounds,
+                                                     out_labels=out_ids, out_dists=out_dists)
+            if self.metric == Metric.EUCLIDEAN:
+                dists.sqrt_()
+            return dists, ids
+        ids = np.full((B, limit), np.iinfo(np.uint64).max, dtype=np.uint64)
+        dists = np.full((B, limit), np.inf, dtype=np.float32)
+
+        def take(rows):
+            if isinstance(queries, np.ndarray):
+                return queries[rows]
+            import torch
+            return queries[torch.as_tensor(rows, device=queries.device)]
+
+        for fid in np.unique(qf.ids[brute]).tolist():
+            rows = np.flatnonzero(brute & (qf.ids == fid))
+            k = int(k_row[rows[0]])
+            if k <= 0:
+                continue
+            self._index.set_ef(max(self.ef_search, k))
+            i, d = self._index._e.scan_subset(take(rows), qf.labels(fid), k=k, normalize=self._normalize_rounds)
+            ids[rows, :k], dists[rows, :k] = i, d
+        walk = ~brute & (k_row > 0)
+        for k in np.unique(k_row[walk]).tolist():
+            rows = np.flatnonzero(walk & (k_row == k))
+            self._index.set_ef(max(self.ef_search, k))
+            i, d = self._index.knn_query_multi(take(rows), qf.ids[rows], k=k, normalize=self._normalize_rounds)
+            ids[rows, :k], dists[rows, :k] = i, d
+        return (np.sqrt(dists) if self.metric == Metric.EUCLIDEAN else dists), ids
+
     def list_filter(self, prepared: PreparedFilter, order_by=None, ascending=True):
         """The admitted labels in CellTable.query's order (annlite/storage/table.py:259-318)."""
         return self.attributes.order(self._index._e, prepared.labels(), order_by, ascending)
@@ -157,15 +275,19 @@ class HnswIndex:
         return dists[0], ids[0]
 
     def search_batch(self, queries, limit: int = 10, indices=None, out_ids=None, out_dists=None,
-                     filter: Optional[PreparedFilter] = None):
+                     filter: Optional[Union[PreparedFilter, QueryFilters]] = None):
         """Batched search: (B, dim) -> (dists (B, limit), ids (B, limit)).  `queries` may be a numpy
         array (host) or a torch CUDA tensor; device outputs can be supplied to stay on the GPU.  `filter` = a
-        PreparedFilter in place of `indices`: the same rules, its count standing in for len(indices)."""
+        PreparedFilter in place of `indices`: the same rules, its count standing in for len(indices).  Or a
+        QueryFilters of B filters: row i is what query i alone with its own filter returns, padded to `limit` with
+        UINT64_MAX / +inf where its filter admits fewer rows."""
         self._ensure_backend()
         if isinstance(queries, np.ndarray) or not hasattr(queries, 'data_ptr'):
             queries = self._prep(queries)
         if filter is not None and indices is not None:
             raise ValueError('pass either indices or a prepared filter')
+        if isinstance(filter, QueryFilters):
+            return self._search_per_query(queries, limit, filter, out_ids=out_ids, out_dists=out_dists)
         n_allowed = filter.count if filter is not None else (len(indices) if indices is not None else None)
         if n_allowed is not None and n_allowed < limit:
             limit = n_allowed
@@ -204,6 +326,17 @@ class HnswIndex:
             queries = self._prep(queries)
         if filter is not None and indices is not None:
             raise ValueError('pass either indices or a prepared filter')
+        if isinstance(filter, QueryFilters):
+            if len(filter) != queries.shape[0]:
+                raise ValueError(f'{len(filter)} filters for {queries.shape[0]} queries')
+            if np.any((filter.counts >= 0) & (filter.counts < limit)):
+                raise ValueError('a filter admits fewer rows than `limit`: use search_batch (it shrinks the limit like '
+                                 'the reference)')
+            from ...._lib import MAX_EF
+            if max(self.ef_search, limit) > MAX_EF:
+                raise ValueError(f'limit / ef_search above {MAX_EF} is not supported by the GPU walk (ANNB_MAX_EF)')
+            self._index.set_ef(max(self.ef_search, limit))
+            return self._index.knn_query_submit_multi(queries, filter.ids, k=limit, normalize=self._normalize_rounds)
         n_allowed = filter.count if filter is not None else (len(indices) if indices is not None else None)
         if n_allowed is not None and n_allowed < limit:
             raise ValueError('fewer allowed ids than `limit`: use search_batch (it shrinks the limit like the reference)')

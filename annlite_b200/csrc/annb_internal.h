@@ -142,6 +142,9 @@ struct SearchParams {
   uint64_t *cand;         // slots * cand_cap  (packed: float bits << 32 | id)
   int cand_cap;
   int32_t *overflow_flag;
+  // per-query filters (annb_search_multi): B bitmaps by internal id, one per query row of this launch (the row qmap
+  // names, for the bitmap walk), nullptr = "not deleted"; nullptr here = every query uses `filter`
+  const uint32_t *const *query_filter;
 };
 
 // ------------------------------------------------------------------------------------------
@@ -168,9 +171,29 @@ struct AttrColDev {
 
 struct PreparedFilter {
   uint32_t *bits = nullptr;  // by-id bitmap, (n+31)/32 + 1 words: the layout of S_FLT_BY_ID
+  std::shared_ptr<void> block;  // the allocation `bits` lies in, shared by the filters of one prepare call
   int64_t n = 0;             // rows it covers (gd.n at prepare time)
   int64_t count = 0;         // admitted rows
   uint64_t gen = 0;          // annb_index::state_gen at prepare time
+};
+
+// a batch with one filter per query (annb_search_multi / annb_search_submit_multi), in its gathered row order: the
+// rows of each routing group are contiguous; gathered row i is the caller's row perm[i]
+struct MultiBatch {
+  int64_t B = 0;
+  int k = 0, ef = 0;
+  const float *dq = nullptr;                 // gathered queries, normalised (B, dim)
+  const uint32_t *const *dqf = nullptr;      // gathered per-query bitmaps (nullptr = no filter)
+  const uint32_t *dperm = nullptr;           // (B) caller row of each gathered row
+  uint64_t *gl = nullptr;                    // gathered outputs (B, k) / (B, k) / (B)
+  float *gd = nullptr;
+  int32_t *gfound = nullptr;
+  uint64_t *dl = nullptr;                    // outputs in the caller's row order, on the device
+  float *dd = nullptr;
+  uint64_t *host_labels = nullptr;           // host outputs, or nullptr (device outputs)
+  float *host_dists = nullptr;
+  int32_t *hfound = nullptr;                 // pinned copy of gfound
+  int table_slot = 0;                        // scratch slot of the K1 tables a re-run builds
 };
 
 // ------------------------------------------------------------------------------------------
@@ -210,8 +233,8 @@ struct annb_index {
   size_t cap_rec0 = 0, cap_up = 0, cap_labels = 0, cap_deleted = 0;
 
   // scratch (grown on demand)
-  void *d_scratch[32] = {nullptr};
-  size_t scratch_cap[32] = {0};
+  void *d_scratch[40] = {nullptr};
+  size_t scratch_cap[40] = {0};
   void *h_pinned[6] = {nullptr};
   size_t pinned_cap[6] = {0};
   // asynchronous submit/wait lanes (annb_search_submit): lane i works on stream i with its own scratch
@@ -231,6 +254,8 @@ struct annb_index {
     int32_t *dfound = nullptr;
     uint64_t *host_labels = nullptr;    // host outputs to refresh after a re-run, or nullptr (device outputs)
     float *host_dists = nullptr;
+    bool multi = false;                 // a per-query filter batch (annb_search_submit_multi): its state is `mb`
+    MultiBatch mb;
   } lanes[2];
   uint32_t next_ticket = 0;
 
@@ -279,9 +304,11 @@ enum {
   S_QUERIES = 0, S_TABLES, S_OUT_D, S_OUT_L, S_COUNTER, S_VISITED, S_TOUCHED, S_CAND,
   S_FOUND, S_STATS, S_FLT_LABELS, S_FLT_BY_LABEL, S_FLT_BY_ID, S_RAW0, S_CODES, S_MISC, S_PART_D, S_PART_I,
   S_L1_QUERIES, S_L1_TABLES, S_L1_OUT_D, S_L1_OUT_L, S_L1_FOUND, S_L0_FOUND, S_LANE_COUNTERS, S_QMAP,
-  S_L1_FLT_LABELS, S_L1_FLT_BY_LABEL, S_L1_FLT_BY_ID, S_FILTER_PROG, S_FILTER_SCAN, S_FILTER_OUT, S_SCRATCH_SLOTS
+  S_L1_FLT_LABELS, S_L1_FLT_BY_LABEL, S_L1_FLT_BY_ID, S_FILTER_PROG, S_FILTER_SCAN, S_FILTER_OUT,
+  S_MULTI0, S_MULTI1,  // per-query filter batches of lane 0 (and the blocking call) / lane 1: MultiBatch buffers
+  S_SCRATCH_SLOTS
 };
-static_assert(S_SCRATCH_SLOTS <= 32, "annb_index::d_scratch is too small");
+static_assert(S_SCRATCH_SLOTS <= 40, "annb_index::d_scratch is too small");
 
 // kernels (launchers)
 int launch_l2_normalize(annb_index *h, float *x, int64_t B, int D);
@@ -316,6 +343,14 @@ int launch_filter_compact(annb_index *h, const uint32_t *d_bits, int64_t n, cons
                           unsigned int *d_block_scratch);
 // blocks launch_filter_compact uses for n rows (its scratch holds one u32 per block)
 int64_t filter_compact_blocks(int64_t n);
+// F validated programs in one pass (filter_eval_kernel<true>): program f = ops [d_offs[f], d_offs[f + 1]) of d_prog,
+// constant offsets rebased into the one pool; bitmap f at d_bits + f * stride_words, its count added to d_counts[f]
+int launch_filter_eval_many(annb_index *h, int F, const annb_filter_op_t *d_prog, const int *d_offs, int n_ops,
+                            const void *d_consts, int n_const_bytes, const AttrColDev *cols, int n_cols, int64_t n,
+                            const uint32_t *d_deleted, uint32_t *d_bits, int64_t stride_words,
+                            unsigned long long *d_counts);
+// rows of `row_words` u32: gather (dst[i] = src[idx[i]]) or scatter (dst[idx[i]] = src[i]) for i < n
+int launch_rows_copy(annb_index *h, const void *src, void *dst, const uint32_t *d_idx, int64_t n, int row_words, bool scatter);
 
 // host builder
 int hnsw_insert_rows(annb_index *h, const uint8_t *codes, const uint64_t *labels, int64_t n, int num_threads,

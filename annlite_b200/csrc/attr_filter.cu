@@ -7,6 +7,9 @@
 // 8-byte (INTEGER / FLOAT) or 4-byte (TEXT code) loads; validity and deletion words are one broadcast load per warp.
 // Bytes moved: n * (sum of the widths of the referenced columns) + validity words + 2 * n / 8 (deleted in, bits out).
 //
+// filter_eval_kernel<true> evaluates F programs in the same pass (annb_filter_prepare_many): a warp runs them one after
+// the other over its 32 rows, so HBM sees about one pass over the referenced columns plus F * n / 8 bytes of bitmaps.
+//
 // filter_compact_kernel turns a bitmap into the labels of its rows in internal-id order: per-block counts, one scan
 // of the block counts, then each block writes its rows at its offset.
 #include <algorithm>
@@ -37,12 +40,79 @@ __device__ __forceinline__ bool sorted_contains(const T *a, int len, T v) {
   return a[base] == v;
 }
 
+// One program over the warp's 32 rows (row = w * 32 + lane): the bool the stack is left with.
+__device__ __forceinline__ bool eval_program(const annb_filter_op_t *sprog, int n_ops, const uint8_t *cbytes,
+                                             const EvalCols &cols, int64_t w, int64_t row, bool in, int lane) {
+  uint32_t stack = 0;
+  int sd = 0;
+  for (int i = 0; i < n_ops; i++) {
+    const annb_filter_op_t o = sprog[i];
+    if (o.op == ANNB_FOP_AND || o.op == ANNB_FOP_OR) {
+      sd--;
+      const uint32_t a = (stack >> (sd - 1)) & 1u, b = (stack >> sd) & 1u;
+      const uint32_t r = o.op == ANNB_FOP_AND ? (a & b) : (a | b);
+      stack = (stack & ~(1u << (sd - 1))) | (r << (sd - 1));
+      continue;
+    }
+    bool r;
+    if (o.op == ANNB_FOP_FALSE) {
+      r = false;
+    } else if (o.op == ANNB_FOP_TRUE) {
+      r = in;
+    } else {
+      const AttrColDev &c = cols.c[o.col];
+      const bool valid = in && ((__ldg(c.valid + w) >> lane) & 1u);
+      switch (o.op) {
+        case ANNB_FOP_NOTNULL: r = valid; break;
+        case ANNB_FOP_INT_RANGE:
+        case ANNB_FOP_INT_NE:
+        case ANNB_FOP_INT_IN:
+        case ANNB_FOP_INT_NIN: {
+          const int64_t v = valid ? __ldg(reinterpret_cast<const long long *>(c.vals) + row) : 0;
+          const int64_t *k = reinterpret_cast<const int64_t *>(cbytes + o.a);
+          if (o.op == ANNB_FOP_INT_RANGE) r = valid && k[0] <= v && v <= k[1];
+          else if (o.op == ANNB_FOP_INT_NE) r = valid && v != k[0];
+          else r = valid && (sorted_contains(k, o.b, v) == (o.op == ANNB_FOP_INT_IN));
+          break;
+        }
+        case ANNB_FOP_FLT_RANGE:
+        case ANNB_FOP_FLT_NE:
+        case ANNB_FOP_FLT_IN:
+        case ANNB_FOP_FLT_NIN: {
+          const double v = valid ? __ldg(reinterpret_cast<const double *>(c.vals) + row) : 0.0;
+          const double *k = reinterpret_cast<const double *>(cbytes + o.a);
+          if (o.op == ANNB_FOP_FLT_RANGE) r = valid && k[0] <= v && v <= k[1];
+          else if (o.op == ANNB_FOP_FLT_NE) r = valid && v != k[0];
+          else r = valid && (sorted_contains(k, o.b, v) == (o.op == ANNB_FOP_FLT_IN));
+          break;
+        }
+        default: {  // ANNB_FOP_CODE_IN
+          const int32_t v = valid ? __ldg(reinterpret_cast<const int *>(c.vals) + row) : -1;
+          const uint32_t *set = reinterpret_cast<const uint32_t *>(cbytes + o.a);
+          r = valid && v >= 0 && v < o.b && ((set[v >> 5] >> (v & 31)) & 1u);
+          break;
+        }
+      }
+    }
+    stack = (stack & ~(1u << sd)) | ((uint32_t)r << sd);
+    sd++;
+  }
+  return stack & 1u;
+}
+
+// MULTI = false: one program (annb_filter_prepare).  MULTI = true: F programs over the same rows in one pass
+// (annb_filter_prepare_many): the programs sit back to back in `prog` (program f = ops [offs[f], offs[f + 1]); their
+// constant offsets already point into the one pool), a warp keeps its 32 rows and runs every program over them, so the
+// column words the later programs read come from L1.  Program f writes the bitmap at bits + f * stride and adds its
+// admitted rows to count[f].
+template <bool MULTI>
 __global__ void __launch_bounds__(kEvalThreads) filter_eval_kernel(const annb_filter_op_t *__restrict__ prog, int n_ops,
                                                                    const uint32_t *__restrict__ consts, int n_const_words,
                                                                    const EvalCols cols, int64_t n,
                                                                    const uint32_t *__restrict__ deleted,
                                                                    uint32_t *__restrict__ bits,
-                                                                   unsigned long long *__restrict__ count) {
+                                                                   unsigned long long *__restrict__ count, int F,
+                                                                   const int *__restrict__ offs, int64_t stride) {
   extern __shared__ __align__(16) uint32_t smem[];
   __shared__ unsigned int block_count;
   annb_filter_op_t *sprog = reinterpret_cast<annb_filter_op_t *>(smem);
@@ -50,6 +120,13 @@ __global__ void __launch_bounds__(kEvalThreads) filter_eval_kernel(const annb_fi
   const uint32_t *gprog = reinterpret_cast<const uint32_t *>(prog);
   for (int i = threadIdx.x; i < n_ops * 4; i += blockDim.x) smem[i] = gprog[i];
   for (int i = threadIdx.x; i < n_const_words; i += blockDim.x) sconst[i] = consts[i];
+  // MULTI: [F + 1 program offsets][F block counts] behind the pool
+  int *soff = reinterpret_cast<int *>(sconst + n_const_words);
+  unsigned int *scount = reinterpret_cast<unsigned int *>(soff + F + 1);
+  if constexpr (MULTI) {
+    for (int i = threadIdx.x; i <= F; i += blockDim.x) soff[i] = offs[i];
+    for (int i = threadIdx.x; i < F; i += blockDim.x) scount[i] = 0;
+  }
   if (threadIdx.x == 0) block_count = 0;
   __syncthreads();
   const uint8_t *cbytes = reinterpret_cast<const uint8_t *>(sconst);
@@ -61,70 +138,37 @@ __global__ void __launch_bounds__(kEvalThreads) filter_eval_kernel(const annb_fi
   for (int64_t w = (((int64_t)blockIdx.x * blockDim.x) + threadIdx.x) >> 5; w < words; w += nwarps) {
     const int64_t row = w * 32 + lane;
     const bool in = row < n;
-    uint32_t stack = 0;
-    int sd = 0;
-    for (int i = 0; i < n_ops; i++) {
-      const annb_filter_op_t o = sprog[i];
-      if (o.op == ANNB_FOP_AND || o.op == ANNB_FOP_OR) {
-        sd--;
-        const uint32_t a = (stack >> (sd - 1)) & 1u, b = (stack >> sd) & 1u;
-        const uint32_t r = o.op == ANNB_FOP_AND ? (a & b) : (a | b);
-        stack = (stack & ~(1u << (sd - 1))) | (r << (sd - 1));
-        continue;
-      }
-      bool r;
-      if (o.op == ANNB_FOP_FALSE) {
-        r = false;
-      } else if (o.op == ANNB_FOP_TRUE) {
-        r = in;
-      } else {
-        const AttrColDev &c = cols.c[o.col];
-        const bool valid = in && ((__ldg(c.valid + w) >> lane) & 1u);
-        switch (o.op) {
-          case ANNB_FOP_NOTNULL: r = valid; break;
-          case ANNB_FOP_INT_RANGE:
-          case ANNB_FOP_INT_NE:
-          case ANNB_FOP_INT_IN:
-          case ANNB_FOP_INT_NIN: {
-            const int64_t v = valid ? __ldg(reinterpret_cast<const long long *>(c.vals) + row) : 0;
-            const int64_t *k = reinterpret_cast<const int64_t *>(cbytes + o.a);
-            if (o.op == ANNB_FOP_INT_RANGE) r = valid && k[0] <= v && v <= k[1];
-            else if (o.op == ANNB_FOP_INT_NE) r = valid && v != k[0];
-            else r = valid && (sorted_contains(k, o.b, v) == (o.op == ANNB_FOP_INT_IN));
-            break;
-          }
-          case ANNB_FOP_FLT_RANGE:
-          case ANNB_FOP_FLT_NE:
-          case ANNB_FOP_FLT_IN:
-          case ANNB_FOP_FLT_NIN: {
-            const double v = valid ? __ldg(reinterpret_cast<const double *>(c.vals) + row) : 0.0;
-            const double *k = reinterpret_cast<const double *>(cbytes + o.a);
-            if (o.op == ANNB_FOP_FLT_RANGE) r = valid && k[0] <= v && v <= k[1];
-            else if (o.op == ANNB_FOP_FLT_NE) r = valid && v != k[0];
-            else r = valid && (sorted_contains(k, o.b, v) == (o.op == ANNB_FOP_FLT_IN));
-            break;
-          }
-          default: {  // ANNB_FOP_CODE_IN
-            const int32_t v = valid ? __ldg(reinterpret_cast<const int *>(c.vals) + row) : -1;
-            const uint32_t *set = reinterpret_cast<const uint32_t *>(cbytes + o.a);
-            r = valid && v >= 0 && v < o.b && ((set[v >> 5] >> (v & 31)) & 1u);
-            break;
-          }
+    if constexpr (MULTI) {
+      const bool live = in && !(deleted && ((__ldg(deleted + w) >> lane) & 1u));
+      for (int f = 0; f < F; f++) {
+        const int o0 = soff[f];
+        const bool r = eval_program(sprog + o0, soff[f + 1] - o0, cbytes, cols, w, row, in, lane);
+        const bool keep = live && r;
+        const uint32_t word = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) {
+          bits[f * stride + w] = word;
+          if (word) atomicAdd(&scount[f], (unsigned int)__popc(word));
         }
       }
-      stack = (stack & ~(1u << sd)) | ((uint32_t)r << sd);
-      sd++;
-    }
-    const bool keep = in && (stack & 1u) && !(deleted && ((__ldg(deleted + w) >> lane) & 1u));
-    const uint32_t word = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) {
-      bits[w] = word;
-      mine += __popc(word);
+    } else {
+      const bool r = eval_program(sprog, n_ops, cbytes, cols, w, row, in, lane);
+      const bool keep = in && r && !(deleted && ((__ldg(deleted + w) >> lane) & 1u));
+      const uint32_t word = __ballot_sync(0xffffffffu, keep);
+      if (lane == 0) {
+        bits[w] = word;
+        mine += __popc(word);
+      }
     }
   }
-  if (lane == 0 && mine) atomicAdd(&block_count, mine);
-  __syncthreads();
-  if (threadIdx.x == 0 && block_count) atomicAdd(count, (unsigned long long)block_count);
+  if constexpr (MULTI) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < F; i += blockDim.x)
+      if (scount[i]) atomicAdd(count + i, (unsigned long long)scount[i]);
+  } else {
+    if (lane == 0 && mine) atomicAdd(&block_count, mine);
+    __syncthreads();
+    if (threadIdx.x == 0 && block_count) atomicAdd(count, (unsigned long long)block_count);
+  }
 }
 
 __device__ __forceinline__ unsigned int block_exclusive_scan(unsigned int v, unsigned int *warp_sums, unsigned int *total) {
@@ -198,7 +242,28 @@ __global__ void __launch_bounds__(kCompactThreads) filter_compact_kernel(const u
   }
 }
 
+// per-query filter batches: one warp per row, a lane per 4-byte word
+__global__ void __launch_bounds__(256) rows_copy_kernel(const uint32_t *__restrict__ src, uint32_t *__restrict__ dst,
+                                                        const uint32_t *__restrict__ idx, int64_t n, int row_words,
+                                                        bool scatter) {
+  const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (i >= n) return;
+  const int64_t r = __ldg(idx + i);
+  const uint32_t *s = src + (scatter ? i : r) * row_words;
+  uint32_t *d = dst + (scatter ? r : i) * row_words;
+  for (int j = threadIdx.x & 31; j < row_words; j += 32) d[j] = s[j];
+}
+
 }  // namespace
+
+int launch_rows_copy(annb_index *h, const void *src, void *dst, const uint32_t *d_idx, int64_t n, int row_words, bool scatter) {
+  if (n == 0) return ANNB_OK;
+  rows_copy_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, h->stream>>>((const uint32_t *)src, (uint32_t *)dst, d_idx, n,
+                                                                            row_words, scatter);
+  h->launches++;
+  ANNB_CUDA(cudaGetLastError());
+  return ANNB_OK;
+}
 
 int launch_filter_eval(annb_index *h, const annb_filter_op_t *d_prog, int n_ops, const void *d_consts, int n_const_bytes,
                        const AttrColDev *cols, int n_cols, int64_t n, const uint32_t *d_deleted, uint32_t *d_bits,
@@ -210,8 +275,28 @@ int launch_filter_eval(annb_index *h, const annb_filter_op_t *d_prog, int n_ops,
   const int64_t want = (words * 32 + kEvalThreads - 1) / kEvalThreads;
   const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)h->sm_count * 8));
   const size_t smem = (size_t)n_ops * sizeof(annb_filter_op_t) + (size_t)n_const_bytes;
-  filter_eval_kernel<<<blocks, kEvalThreads, smem, h->stream>>>(d_prog, n_ops, (const uint32_t *)d_consts, n_const_bytes / 4,
-                                                                ec, n, d_deleted, d_bits, d_count);
+  filter_eval_kernel<false><<<blocks, kEvalThreads, smem, h->stream>>>(d_prog, n_ops, (const uint32_t *)d_consts, n_const_bytes / 4,
+                                                                       ec, n, d_deleted, d_bits, d_count, 1, nullptr, 0);
+  h->launches++;
+  ANNB_CUDA(cudaGetLastError());
+  return ANNB_OK;
+}
+
+int launch_filter_eval_many(annb_index *h, int F, const annb_filter_op_t *d_prog, const int *d_offs, int n_ops,
+                            const void *d_consts, int n_const_bytes, const AttrColDev *cols, int n_cols, int64_t n,
+                            const uint32_t *d_deleted, uint32_t *d_bits, int64_t stride_words,
+                            unsigned long long *d_counts) {
+  EvalCols ec;
+  memset(&ec, 0, sizeof(ec));
+  for (int i = 0; i < n_cols && i < ANNB_MAX_ATTR_COLUMNS; i++) ec.c[i] = cols[i];
+  const int64_t words = (n + 31) / 32 + 1;
+  const int64_t want = (words * 32 + kEvalThreads - 1) / kEvalThreads;
+  const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)h->sm_count * 8));
+  const size_t smem = (size_t)n_ops * sizeof(annb_filter_op_t) + (size_t)n_const_bytes + (size_t)(2 * F + 1) * 4;
+  if (smem > 48 * 1024)
+    ANNB_CUDA(cudaFuncSetAttribute(filter_eval_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  filter_eval_kernel<true><<<blocks, kEvalThreads, smem, h->stream>>>(d_prog, n_ops, (const uint32_t *)d_consts, n_const_bytes / 4,
+                                                                      ec, n, d_deleted, d_bits, d_counts, F, d_offs, stride_words);
   h->launches++;
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;

@@ -195,8 +195,7 @@ int annb_destroy(annb_index_t *h) {
     if (c.d_vals) cudaFree(c.d_vals);
     if (c.d_valid) cudaFree(c.d_valid);
   }
-  for (auto &f : h->filters)
-    if (f.second.bits) cudaFree(f.second.bits);
+  h->filters.clear();  // the bitmaps live in shared blocks: the last filter of a block frees it
   for (int i = 0; i < 6; i++)
     if (h->ev[i]) cudaEventDestroy(h->ev[i]);
   if (h->stream2) cudaStreamDestroy(h->stream2);
@@ -1324,9 +1323,18 @@ int annb_scan_subset(annb_index_t *h, const float *queries, int in_space, int64_
 // ---- streaming submit / wait ---------------------------------------------------------------------
 // A filtered / deletion-aware batch whose walk flagged queries (found = -1: N outgrew its capacity) is finished at
 // wait time: exactly those queries are re-run on the bitmap walk, on the lane's own stream and scratch.
+static int multi_rerun(annb_index *h, MultiBatch &mb, int64_t n_over);
+
 static int lane_rerun_flagged(annb_index *h, int lane, int64_t n_over) {
   annb_index::AsyncLane &L = h->lanes[lane];
   cudaStream_t st = lane ? h->stream2 : h->stream;
+  if (L.multi) {
+    cudaStream_t saved = h->stream;
+    h->stream = st;
+    const int rc = multi_rerun(h, L.mb, n_over);
+    h->stream = saved;
+    return rc;
+  }
   uint32_t *hmap, *dmap;
   float *t;
   ANNB_TRY(annb_pinned(h, 3, (size_t)n_over * 4, (void **)&hmap));
@@ -1527,6 +1535,7 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   L.dfound = dfound;
   L.host_labels = host_out ? labels_out : nullptr;
   L.host_dists = host_out ? dists_out : nullptr;
+  L.multi = false;
   *ticket_out = ticket;
   return ANNB_OK;
 }
@@ -1738,6 +1747,137 @@ static int find_filter(annb_index *h, int filter_id, PreparedFilter **out) {
   return ANNB_OK;
 }
 
+// F programs given back to back -> F prepared filters.  Everything is validated first; the referenced columns are
+// synced once; the programs are packed into as few evaluator launches as the LAUNCH limits allow (a launch of one
+// program takes filter_eval_kernel<false>, the single-filter kernel), all uploaded in one copy; one synchronisation.
+// The F bitmaps share one allocation.
+static int prepare_many_impl(annb_index *h, int F, const annb_filter_op_t *programs, const int *n_ops, const void *consts,
+                             const int64_t *n_const_bytes, int *filter_ids, int64_t *counts) {
+  std::vector<int64_t> op0((size_t)F + 1, 0), c0((size_t)F + 1, 0);
+  for (int f = 0; f < F; f++) {
+    if (n_ops[f] < 0 || n_const_bytes[f] < 0) ANNB_FAIL(ANNB_EINVAL, "filter %d: negative size", f);
+    op0[f + 1] = op0[f] + n_ops[f];
+    c0[f + 1] = c0[f] + n_const_bytes[f];
+  }
+  const uint8_t *cbase = (const uint8_t *)consts;
+  for (int f = 0; f < F; f++) {
+    if (n_const_bytes[f] > 0 && !consts) ANNB_FAIL(ANNB_EINVAL, "filter %d: null constants", f);
+    const int rc = validate_program(h, programs + op0[f], n_ops[f], n_const_bytes[f] ? cbase + c0[f] : nullptr, n_const_bytes[f]);
+    if (rc != ANNB_OK) {
+      if (F > 1) {
+        const std::string msg = annb_last_error();
+        annb_set_error("filter %d: %s", f, msg.c_str());
+      }
+      return rc;
+    }
+  }
+  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
+  ANNB_TRY(drain_lanes(h));
+  ANNB_TRY(sync_device_graph(h));
+  attr_fit(h);
+  const int64_t n = h->gd.n;
+  std::vector<AttrColDev> cols(h->attrs.size());
+  std::vector<char> used(h->attrs.size(), 0);
+  for (int64_t i = 0; i < op0[F]; i++)
+    if (programs[i].op != ANNB_FOP_AND && programs[i].op != ANNB_FOP_OR && programs[i].op > ANNB_FOP_TRUE) used[programs[i].col] = 1;
+  for (size_t c = 0; c < h->attrs.size(); c++) {
+    if (!used[c]) continue;
+    ANNB_TRY(attr_sync_dev(h, h->attrs[c], n));
+    cols[c] = AttrColDev{h->attrs[c].d_vals, h->attrs[c].d_valid, h->attrs[c].type};
+  }
+  // launches: consecutive programs while their ops and constants fit one launch's shared memory (a single program
+  // always fits: ANNB_FILTER_MAX_OPS / _CONST_BYTES are below the LAUNCH limits)
+  struct Launch {
+    int f0, f1;
+    size_t prog, offs, consts;  // byte offsets in the upload
+    int ops, cbytes;
+  };
+  auto up16 = [](size_t x) { return (x + 15) / 16 * 16; };
+  std::vector<Launch> launches;
+  for (int f = 0; f < F;) {
+    Launch l{f, f, 0, 0, 0, 0, 0};
+    while (l.f1 < F && (l.f1 == l.f0 || (l.ops + n_ops[l.f1] <= ANNB_FILTER_LAUNCH_MAX_OPS &&
+                                          l.cbytes + n_const_bytes[l.f1] <= ANNB_FILTER_LAUNCH_MAX_CONST_BYTES))) {
+      l.ops += n_ops[l.f1];
+      l.cbytes += (int)n_const_bytes[l.f1];
+      l.f1++;
+    }
+    launches.push_back(l);
+    f = l.f1;
+  }
+  size_t total = 0;
+  for (Launch &l : launches) {
+    l.prog = total;
+    total = up16(total + (size_t)l.ops * sizeof(annb_filter_op_t));
+    l.consts = total;
+    total = up16(total + (size_t)l.cbytes);
+    l.offs = total;
+    total = up16(total + (size_t)(l.f1 - l.f0 + 1) * 4);
+  }
+  const size_t counts_at = total;
+  total += (size_t)F * 8;
+  std::vector<uint8_t> up(total, 0);
+  for (const Launch &l : launches) {
+    annb_filter_op_t *dst = reinterpret_cast<annb_filter_op_t *>(up.data() + l.prog);
+    int *offs = reinterpret_cast<int *>(up.data() + l.offs);
+    int at = 0, cat = 0;
+    for (int f = l.f0; f < l.f1; f++) {
+      offs[f - l.f0] = at;
+      for (int i = 0; i < n_ops[f]; i++) {
+        annb_filter_op_t o = programs[op0[f] + i];
+        if (o.op >= ANNB_FOP_INT_RANGE && o.op <= ANNB_FOP_CODE_IN) o.a += cat;  // into the launch's one pool
+        dst[at++] = o;
+      }
+      if (n_const_bytes[f]) memcpy(up.data() + l.consts + cat, cbase + c0[f], (size_t)n_const_bytes[f]);
+      cat += (int)n_const_bytes[f];
+    }
+    offs[l.f1 - l.f0] = at;
+  }
+  uint8_t *dbuf;
+  ANNB_TRY(annb_scratch(h, S_FILTER_PROG, total, (void **)&dbuf));
+  unsigned long long *dcounts = (unsigned long long *)(dbuf + counts_at);
+  const int64_t words = (n + 31) / 32 + 1, stride = (words + 3) / 4 * 4;  // bitmaps 16-byte aligned
+  void *block = nullptr;
+  ANNB_CUDA(cudaMalloc(&block, (size_t)stride * 4 * F));
+  std::shared_ptr<void> owner(block, [](void *p) { cudaFree(p); });
+  uint32_t *bits = (uint32_t *)block;
+  int rc = ANNB_OK;
+  std::vector<unsigned long long> hcounts((size_t)F, 0);
+  if (cudaMemcpyAsync(dbuf, up.data(), counts_at, cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
+      cudaMemsetAsync(dcounts, 0, (size_t)F * 8, h->stream) != cudaSuccess)
+    rc = ANNB_ECUDA;
+  for (size_t i = 0; i < launches.size() && rc == ANNB_OK; i++) {
+    const Launch &l = launches[i];
+    const annb_filter_op_t *dprog = (const annb_filter_op_t *)(dbuf + l.prog);
+    if (l.f1 - l.f0 == 1)
+      rc = launch_filter_eval(h, dprog, l.ops, dbuf + l.consts, l.cbytes, cols.data(), (int)cols.size(), n, h->gd.deleted,
+                              bits + (size_t)l.f0 * stride, dcounts + l.f0);
+    else
+      rc = launch_filter_eval_many(h, l.f1 - l.f0, dprog, (const int *)(dbuf + l.offs), l.ops, dbuf + l.consts, l.cbytes, cols.data(),
+                                   (int)cols.size(), n, h->gd.deleted, bits + (size_t)l.f0 * stride, stride, dcounts + l.f0);
+  }
+  if (rc == ANNB_OK && (cudaMemcpyAsync(hcounts.data(), dcounts, (size_t)F * 8, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
+                        cudaStreamSynchronize(h->stream) != cudaSuccess))
+    rc = ANNB_ECUDA;
+  if (rc != ANNB_OK) {
+    if (rc == ANNB_ECUDA) annb_set_error("CUDA error while evaluating a filter: %s", cudaGetErrorString(cudaGetLastError()));
+    return rc;
+  }
+  for (int f = 0; f < F; f++) {
+    PreparedFilter pf;
+    pf.bits = bits + (size_t)f * stride;
+    pf.block = owner;
+    pf.n = n;
+    pf.count = (int64_t)hcounts[f];
+    pf.gen = h->state_gen;
+    const int id = h->next_filter_id++;
+    h->filters[id] = pf;
+    filter_ids[f] = id;
+    counts[f] = pf.count;
+  }
+  return ANNB_OK;
+}
+
 extern "C" {
 
 int annb_attr_define(annb_index_t *h, int col, int type) {
@@ -1843,53 +1983,20 @@ int annb_filter_prepare(annb_index_t *h, const annb_filter_op_t *program, int n_
   if (!filter_id || !count) ANNB_FAIL(ANNB_EINVAL, "null outputs");
   *filter_id = 0;
   *count = 0;
-  ANNB_TRY(validate_program(h, program, n_ops, consts, n_const_bytes));
-  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
-  ANNB_TRY(drain_lanes(h));
-  ANNB_TRY(sync_device_graph(h));
-  attr_fit(h);
-  const int64_t n = h->gd.n;
-  std::vector<AttrColDev> cols(h->attrs.size());
-  std::vector<char> used(h->attrs.size(), 0);
-  for (int i = 0; i < n_ops; i++)
-    if (program[i].op != ANNB_FOP_AND && program[i].op != ANNB_FOP_OR && program[i].op > ANNB_FOP_TRUE) used[program[i].col] = 1;
-  for (size_t c = 0; c < h->attrs.size(); c++) {
-    if (!used[c]) continue;
-    ANNB_TRY(attr_sync_dev(h, h->attrs[c], n));
-    cols[c] = AttrColDev{h->attrs[c].d_vals, h->attrs[c].d_valid, h->attrs[c].type};
+  return prepare_many_impl(h, 1, program, &n_ops, consts, &n_const_bytes, filter_id, count);
+}
+
+int annb_filter_prepare_many(annb_index_t *h, int F, const annb_filter_op_t *programs, const int *n_ops, const void *consts,
+                             const int64_t *n_const_bytes, int *filter_ids_out, int64_t *counts_out) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  if (F <= 0 || !programs || !n_ops || !n_const_bytes || !filter_ids_out || !counts_out) ANNB_FAIL(ANNB_EINVAL, "bad arguments");
+  if (F > ANNB_FILTER_MAX_PER_CALL) ANNB_FAIL(ANNB_ELIMIT, "%d filters in one call (limit %d)", F, ANNB_FILTER_MAX_PER_CALL);
+  for (int f = 0; f < F; f++) {
+    filter_ids_out[f] = 0;
+    counts_out[f] = 0;
   }
-  const size_t words = (size_t)(n + 31) / 32 + 1;
-  const size_t pbytes = (size_t)n_ops * sizeof(annb_filter_op_t);
-  uint8_t *dprog;
-  ANNB_TRY(annb_scratch(h, S_FILTER_PROG, pbytes + (size_t)n_const_bytes + 16, (void **)&dprog));
-  unsigned long long *dcount = (unsigned long long *)(dprog + pbytes + n_const_bytes);  // both multiples of 8
-  PreparedFilter f;
-  f.n = n;
-  f.gen = h->state_gen;
-  ANNB_CUDA(cudaMalloc(&f.bits, words * 4));
-  int rc = ANNB_OK;
-  unsigned long long hcount = 0;
-  if (cudaMemcpyAsync(dprog, program, pbytes, cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-      (n_const_bytes && cudaMemcpyAsync(dprog + pbytes, consts, (size_t)n_const_bytes, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) ||
-      cudaMemsetAsync(dcount, 0, 8, h->stream) != cudaSuccess)
-    rc = ANNB_ECUDA;
-  if (rc == ANNB_OK)
-    rc = launch_filter_eval(h, (const annb_filter_op_t *)dprog, n_ops, dprog + pbytes, (int)n_const_bytes, cols.data(), (int)cols.size(),
-                            n, h->gd.deleted, f.bits, dcount);
-  if (rc == ANNB_OK && (cudaMemcpyAsync(&hcount, dcount, 8, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
-                        cudaStreamSynchronize(h->stream) != cudaSuccess))
-    rc = ANNB_ECUDA;
-  if (rc != ANNB_OK) {
-    cudaFree(f.bits);
-    if (rc == ANNB_ECUDA) annb_set_error("CUDA error while evaluating a filter: %s", cudaGetErrorString(cudaGetLastError()));
-    return rc;
-  }
-  f.count = (int64_t)hcount;
-  const int id = h->next_filter_id++;
-  h->filters[id] = f;
-  *filter_id = id;
-  *count = f.count;
-  return ANNB_OK;
+  return prepare_many_impl(h, F, programs, n_ops, consts, n_const_bytes, filter_ids_out, counts_out);
 }
 
 int annb_filter_labels(annb_index_t *h, int filter_id, uint64_t *labels_out, int64_t cap, int64_t *n_out) {
@@ -1916,8 +2023,7 @@ int annb_filter_release(annb_index_t *h, int filter_id) {
   auto it = h->filters.find(filter_id);
   if (it == h->filters.end()) ANNB_FAIL(ANNB_EINVAL, "no prepared filter %d", filter_id);
   ANNB_TRY(drain_lanes(h));  // a streamed batch may still walk (or re-run on) this bitmap
-  if (it->second.bits) ANNB_CUDA(cudaFree(it->second.bits));
-  h->filters.erase(it);
+  h->filters.erase(it);      // frees the block once no filter of its prepare call is left
   return ANNB_OK;
 }
 
@@ -1938,6 +2044,301 @@ int annb_search_submit_prepared(annb_index_t *h, const float *queries, int in_sp
   PreparedFilter *f;
   ANNB_TRY(find_filter(h, filter_id, &f));
   return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, f, labels_out, dists_out, out_space, ticket_out);
+}
+
+// ---- per-query filters ----------------------------------------------------------------------------------
+// A batch with one filter per query is split into three routing groups, each ONE launch over its rows gathered into a
+// contiguous block: 0 = no filter (the plain walk, or the deletion-aware one), 1 = filters hnsw_walk4f takes (its list
+// N sized by the group's smallest selectivity, so one selective filter does not move every query to the round-1
+// kernel), 2 = the other filtered rows (hnsw_walk_flagged / the bitmap walk).  Each walk reads query q's bitmap from
+// the per-query table; queries any walk flagged are re-run on the bitmap walk with their own bitmap.
+struct MultiGroup {
+  int64_t o = 0, n = 0;  // gathered rows [o, o + n)
+  bool filtered = false;
+  double s = 1.0;        // the selectivity the group's lists are sized by
+  int mode = 0;          // launch_search mode
+  bool fuse = false;     // tables built inside the walk (else K1 first)
+};
+
+// the route annb_search_prepared / annb_search take for the same rows, group by group
+static int multi_plan(annb_index *h, int64_t B, int ef_eff, const int *query_filter, std::vector<uint32_t> &perm,
+                      std::vector<const uint32_t *> &qf, MultiGroup grp[3]) {
+  const double nn = (double)std::max<int64_t>(1, h->gd.n);
+  std::unordered_map<int, std::pair<const PreparedFilter *, int>> seen;  // id -> (filter, group)
+  std::vector<int8_t> which((size_t)B);
+  std::vector<const uint32_t *> bits((size_t)B, nullptr);
+  double smin[3] = {1.0, 1.0, 1.0};
+  int64_t cnt[3] = {0, 0, 0};
+  for (int64_t b = 0; b < B; b++) {
+    const int id = query_filter[b];
+    int g = 0;
+    if (id != 0) {
+      auto it = seen.find(id);
+      if (it == seen.end()) {
+        PreparedFilter *pf;
+        ANNB_TRY(find_filter(h, id, &pf));
+        const double s = std::min<double>(1.0, (double)pf->count / nn);
+        g = (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, s)) ? 1 : 2;
+        smin[g] = std::min(smin[g], s);
+        it = seen.emplace(id, std::make_pair((const PreparedFilter *)pf, g)).first;
+      }
+      g = it->second.second;
+      bits[(size_t)b] = it->second.first->bits;
+    }
+    which[(size_t)b] = (int8_t)g;
+    cnt[g]++;
+  }
+  int64_t at[3] = {0, cnt[0], cnt[0] + cnt[1]};
+  perm.resize((size_t)B);
+  qf.resize((size_t)B);
+  for (int g = 0; g < 3; g++) {
+    grp[g].o = at[g];
+    grp[g].n = cnt[g];
+  }
+  for (int64_t b = 0; b < B; b++) {
+    const int64_t pos = at[which[(size_t)b]]++;
+    perm[(size_t)pos] = (uint32_t)b;
+    qf[(size_t)pos] = bits[(size_t)b];
+  }
+  const bool can_fuse = walk4_can_fuse(h);
+  {  // no filter: search_impl with filter_labels == NULL
+    MultiGroup &g = grp[0];
+    const bool general = h->g.num_deleted > 0 || h->opt_force_general;
+    g.s = 1.0 - (double)h->g.num_deleted / nn;
+    g.mode = general ? (h->opt_force_general == 2 ? 2 : 1) : 0;
+    g.fuse = can_fuse && (!general || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s)));
+  }
+  for (int i = 1; i < 3; i++) {  // a prepared filter: the filtered route
+    MultiGroup &g = grp[i];
+    g.filtered = true;
+    g.s = smin[i];
+    g.mode = h->opt_force_general == 2 ? 2 : 1;
+    g.fuse = can_fuse && h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s);
+  }
+  return ANNB_OK;
+}
+
+// Enqueue a planned batch on h->stream with the scratch of `lane` (0 also serves the blocking call): gather the
+// queries, normalise, one walk per group, scatter the outputs back to the caller's rows, copy `found` (gathered order)
+// and host outputs back.  *flagged = some walk may have flagged queries for a re-run.
+static int multi_enqueue(annb_index *h, int lane, const float *queries, int in_space, int64_t B, int normalize, int k, int ef_eff,
+                         const std::vector<uint32_t> &perm, const std::vector<const uint32_t *> &qf, const MultiGroup grp[3],
+                         uint64_t *labels_out, float *dists_out, int out_space, int pinned_slot, unsigned int *counters,
+                         bool timing, MultiBatch &mb, bool *flagged) {
+  const bool host_in = in_space != ANNB_DEVICE, host_out = out_space != ANNB_DEVICE;
+  const size_t TS = (size_t)h->M * h->Ks, dim = (size_t)h->dim;
+  bool need_tables = false;
+  *flagged = false;
+  for (int g = 0; g < 3; g++) {
+    if (grp[g].n && !grp[g].fuse) need_tables = true;
+    if (grp[g].n && grp[g].mode != 0) *flagged = true;
+  }
+  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t o_perm = al((size_t)B * 8), o_found = o_perm + al((size_t)B * 4), o_gl = o_found + al((size_t)B * 4),
+               o_gd = o_gl + al((size_t)B * k * 8), o_q = o_gd + al((size_t)B * k * 4), total = o_q + al((size_t)B * dim * 4);
+  // all scratch first: a (re)allocation synchronises both lanes, which is only safe before enqueuing
+  uint8_t *mq;
+  ANNB_TRY(annb_scratch(h, lane ? S_MULTI1 : S_MULTI0, total, (void **)&mq));
+  float *draw = nullptr, *dtab = nullptr;
+  if (host_in) ANNB_TRY(annb_scratch(h, lane ? S_L1_QUERIES : S_QUERIES, (size_t)B * dim * 4, (void **)&draw));
+  if (need_tables) ANNB_TRY(annb_scratch(h, lane ? S_L1_TABLES : S_TABLES, (size_t)B * TS * 4, (void **)&dtab));
+  uint64_t *dl = labels_out;
+  float *dd = dists_out;
+  if (host_out) {
+    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_L : S_OUT_L, (size_t)B * k * 8, (void **)&dl));
+    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_D : S_OUT_D, (size_t)B * k * 4, (void **)&dd));
+  }
+  int32_t *hfound;
+  ANNB_TRY(annb_pinned(h, pinned_slot, (size_t)B * 4, (void **)&hfound));
+  std::vector<uint8_t> meta(o_found, 0);
+  memcpy(meta.data(), qf.data(), (size_t)B * 8);
+  memcpy(meta.data() + o_perm, perm.data(), (size_t)B * 4);
+  mb = MultiBatch();
+  mb.B = B;
+  mb.k = k;
+  mb.ef = ef_eff;
+  mb.dqf = reinterpret_cast<const uint32_t *const *>(mq);
+  mb.dperm = reinterpret_cast<const uint32_t *>(mq + o_perm);
+  mb.gfound = reinterpret_cast<int32_t *>(mq + o_found);
+  mb.gl = reinterpret_cast<uint64_t *>(mq + o_gl);
+  mb.gd = reinterpret_cast<float *>(mq + o_gd);
+  float *dq = reinterpret_cast<float *>(mq + o_q);
+  mb.dq = dq;
+  mb.dl = dl;
+  mb.dd = dd;
+  mb.host_labels = host_out ? labels_out : nullptr;
+  mb.host_dists = host_out ? dists_out : nullptr;
+  mb.hfound = hfound;
+  mb.table_slot = lane ? S_L1_TABLES : S_TABLES;
+
+  int rc = ANNB_OK;
+  const float *src = queries;
+  if (cudaMemcpyAsync(mq, meta.data(), o_found, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) rc = ANNB_ECUDA;
+  if (rc == ANNB_OK && host_in) {
+    if (cudaMemcpyAsync(draw, queries, (size_t)B * dim * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) rc = ANNB_ECUDA;
+    src = draw;
+  }
+  if (rc == ANNB_OK) rc = launch_rows_copy(h, src, dq, mb.dperm, B, (int)dim, false);
+  for (int r = 0; r < normalize && rc == ANNB_OK; r++) rc = launch_l2_normalize(h, dq, B, (int)dim);
+  if (rc == ANNB_OK && timing) cudaEventRecord(h->ev[2], h->stream);
+  for (int gi = 0; gi < 3 && rc == ANNB_OK; gi++) {
+    const MultiGroup &g = grp[gi];
+    if (g.n == 0) continue;
+    if (!g.fuse) rc = launch_adc_table(h, dq + g.o * dim, g.n, dtab + g.o * TS);
+    if (rc != ANNB_OK) break;
+    SearchParams p;
+    memset(&p, 0, sizeof(p));
+    if (g.fuse) fuse_params(h, p, dq + g.o * dim);
+    else p.tables = dtab + g.o * TS;
+    p.B = g.n;
+    p.k = k;
+    p.ef = ef_eff;
+    p.query_filter = g.filtered ? mb.dqf + g.o : nullptr;
+    p.selectivity = (float)g.s;
+    p.out_labels = mb.gl + g.o * k;
+    p.out_dists = mb.gd + g.o * k;
+    p.out_found = mb.gfound + g.o;
+    p.work_counter = counters;
+    rc = launch_search(h, p, g.mode);
+  }
+  if (rc == ANNB_OK && timing) cudaEventRecord(h->ev[3], h->stream);
+  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gl, dl, mb.dperm, B, 2 * k, true);
+  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gd, dd, mb.dperm, B, k, true);
+  if (rc == ANNB_OK) {
+    cudaMemcpyAsync(hfound, mb.gfound, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream);
+    if (host_out) {
+      cudaMemcpyAsync(labels_out, dl, (size_t)B * k * 8, cudaMemcpyDeviceToHost, h->stream);
+      cudaMemcpyAsync(dists_out, dd, (size_t)B * k * 4, cudaMemcpyDeviceToHost, h->stream);
+    }
+    if (cudaGetLastError() != cudaSuccess) rc = ANNB_ECUDA;
+  }
+  if (rc == ANNB_ECUDA) annb_set_error("CUDA error while enqueuing a per-query filter search: %s", cudaGetErrorString(cudaGetLastError()));
+  return rc;
+}
+
+// the flagged queries of a settled batch (found = -1) re-run on the bitmap walk with their own bitmaps, on h->stream;
+// then the outputs are scattered and copied back again
+static int multi_rerun(annb_index *h, MultiBatch &mb, int64_t n_over) {
+  uint32_t *hmap, *dmap;
+  float *t;
+  ANNB_TRY(annb_pinned(h, 3, (size_t)n_over * 4, (void **)&hmap));
+  ANNB_TRY(annb_scratch(h, S_QMAP, (size_t)n_over * 4, (void **)&dmap));
+  ANNB_TRY(annb_scratch(h, mb.table_slot, (size_t)mb.B * h->M * h->Ks * sizeof(float), (void **)&t));
+  int64_t w = 0;
+  for (int64_t b = 0; b < mb.B; b++)
+    if (mb.hfound[b] < 0) hmap[w++] = (uint32_t)b;
+  int rc = ANNB_OK;
+  if (cudaMemcpyAsync(dmap, hmap, (size_t)n_over * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) rc = ANNB_ECUDA;
+  if (rc == ANNB_OK) rc = launch_adc_table(h, mb.dq, mb.B, t);
+  if (rc == ANNB_OK) {
+    SearchParams p;
+    memset(&p, 0, sizeof(p));
+    p.tables = t;
+    p.B = n_over;
+    p.k = mb.k;
+    p.ef = mb.ef;
+    p.query_filter = mb.dqf;
+    p.selectivity = 1.f;
+    p.out_labels = mb.gl;
+    p.out_dists = mb.gd;
+    p.out_found = mb.gfound;
+    p.qmap = dmap;
+    rc = launch_search(h, p, 2);
+  }
+  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gl, mb.dl, mb.dperm, mb.B, 2 * mb.k, true);
+  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gd, mb.dd, mb.dperm, mb.B, mb.k, true);
+  if (rc == ANNB_OK) {
+    cudaMemcpyAsync(mb.hfound, mb.gfound, (size_t)mb.B * 4, cudaMemcpyDeviceToHost, h->stream);
+    if (mb.host_labels) {
+      cudaMemcpyAsync(mb.host_labels, mb.dl, (size_t)mb.B * mb.k * 8, cudaMemcpyDeviceToHost, h->stream);
+      cudaMemcpyAsync(mb.host_dists, mb.dd, (size_t)mb.B * mb.k * 4, cudaMemcpyDeviceToHost, h->stream);
+    }
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) rc = ANNB_ECUDA;
+  }
+  if (rc == ANNB_ECUDA) annb_set_error("CUDA error while re-running flagged queries of a per-query filter search: %s",
+                                       cudaGetErrorString(cudaGetLastError()));
+  if (rc != ANNB_OK) return rc;
+  h->flagged_fallbacks++;
+  h->flagged_fallback_queries += n_over;
+  return ANNB_OK;
+}
+
+int annb_search_multi(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
+                      const int *query_filter, uint64_t *labels_out, float *dists_out, int out_space) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  ANNB_TRY(settle_flagged_lanes(h));
+  if (B < 0 || k <= 0 || ef <= 0 || (B > 0 && (!queries || !query_filter || !labels_out || !dists_out)))
+    ANNB_FAIL(ANNB_EINVAL, "bad arguments");
+  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
+  if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
+  ANNB_TRY(sync_device_graph(h));
+  if (B == 0) return ANNB_OK;
+  const int ef_eff = std::max(ef, k);  // hnswalg.h:1279
+  if (ef_eff > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, k)=%d exceeds ANNB_MAX_EF=%d", ef_eff, ANNB_MAX_EF);
+  std::vector<uint32_t> perm;
+  std::vector<const uint32_t *> qf;
+  MultiGroup grp[3];
+  ANNB_TRY(multi_plan(h, B, ef_eff, query_filter, perm, qf, grp));
+  if (h->gd.n == 0) ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+  MultiBatch mb;
+  bool flagged = false;
+  ANNB_TRY(multi_enqueue(h, 0, queries, in_space, B, normalize, k, ef_eff, perm, qf, grp, labels_out, dists_out, out_space, 2,
+                         nullptr, h->opt_timing != 0, mb, &flagged));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  if (flagged) {
+    int64_t n_over = 0;
+    for (int64_t b = 0; b < B; b++) n_over += mb.hfound[b] < 0;
+    if (n_over) ANNB_TRY(multi_rerun(h, mb, n_over));
+  }
+  for (int64_t b = 0; b < B; b++)
+    if (mb.hfound[b] < k)
+      ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+  return ANNB_OK;
+}
+
+int annb_search_submit_multi(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
+                             const int *query_filter, uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  if (!queries || !query_filter || !labels_out || !dists_out || !ticket_out || B <= 0 || k <= 0 || ef <= 0)
+    ANNB_FAIL(ANNB_EINVAL, "bad arguments");
+  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
+  if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
+  if (h->opt_force_general == 2) ANNB_FAIL(ANNB_EINVAL, "streamed searches do not run on the bitmap walk: use annb_search");
+  if (h->dev_dirty || h->deleted_dirty || h->patch_pending) {  // re-upload of the graph: nothing may be in flight
+    ANNB_TRY(lane_wait(h, 0));
+    ANNB_TRY(lane_wait(h, 1));
+    ANNB_TRY(sync_device_graph(h));
+  }
+  if (h->gd.n == 0) ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+  const int ef_eff = std::max(ef, k);
+  if (ef_eff > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, k)=%d exceeds ANNB_MAX_EF=%d", ef_eff, ANNB_MAX_EF);
+  std::vector<uint32_t> perm;
+  std::vector<const uint32_t *> qf;
+  MultiGroup grp[3];
+  ANNB_TRY(multi_plan(h, B, ef_eff, query_filter, perm, qf, grp));
+  const int ticket = (int)(h->next_ticket++ & 0x3fffffff);
+  const int lane = ticket & 1;
+  ANNB_TRY(lane_wait(h, lane));  // a lane holds one batch at a time
+  unsigned int *counters;
+  ANNB_TRY(annb_scratch(h, S_LANE_COUNTERS, 512, (void **)&counters));
+  annb_index::AsyncLane &L = h->lanes[lane];
+  cudaStream_t saved = h->stream;
+  h->stream = lane ? h->stream2 : saved;
+  bool flagged = false;
+  const int rc = multi_enqueue(h, lane, queries, in_space, B, normalize, k, ef_eff, perm, qf, grp, labels_out, dists_out, out_space,
+                               4 + lane, counters + 64 * lane, false, L.mb, &flagged);
+  h->stream = saved;
+  if (rc != ANNB_OK) return rc;
+  L.busy = true;
+  L.B = B;
+  L.k = k;
+  L.hfound = L.mb.hfound;
+  L.flagged = flagged;
+  L.multi = true;
+  *ticket_out = ticket;
+  return ANNB_OK;
 }
 
 }  // extern "C"

@@ -575,7 +575,8 @@ __global__ void hnsw_walk_fast(const GraphDev g, const SearchParams p, const int
 constexpr uint32_t PASS_BIT = 0x40000000u;
 constexpr uint32_t ID_MASK30 = 0x3fffffffu;
 
-template <int EPL, int CR, int CB>
+// PQF: query q is admitted by its own bitmap p.query_filter[q] (nullptr = "not deleted"), chosen per query
+template <int EPL, int CR, int CB, bool PQF>
 __global__ void hnsw_walk_flagged(const GraphDev g, const SearchParams p, const int has_del, const int table_stride_bytes) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -599,7 +600,7 @@ __global__ void hnsw_walk_flagged(const GraphDev g, const SearchParams p, const 
   const unsigned le_mask = lt_mask | (1u << lane);
   constexpr int CW = CR / 4;
   const uint32_t *filter = p.filter;
-  const bool use_filter = filter != nullptr;
+  bool use_filter = filter != nullptr;
   const uint32_t *delbits = g.deleted;
   auto passes = [&](uint32_t id) -> bool {
     if (use_filter) return (__ldg(filter + (id >> 5)) >> (id & 31)) & 1u;   // :353-354, :423-426
@@ -610,6 +611,10 @@ __global__ void hnsw_walk_flagged(const GraphDev g, const SearchParams p, const 
   for (;;) {
     const int64_t q = next_query(p.work_counter, lane);
     if (q >= p.B) break;
+    if constexpr (PQF) {
+      filter = p.query_filter[q];
+      use_filter = filter != nullptr;
+    }
     __syncwarp();
     if (tma_table) {
       if (lane == 0) {
@@ -906,7 +911,8 @@ __device__ __forceinline__ uint32_t cand_id(uint64_t c) { return (uint32_t)c; }
 
 constexpr int SBAG = 256;  // candidate bag entries kept in shared memory per warp (spills to global beyond)
 
-template <int EPL, int CR, int CB, bool SMEM_TABLE>
+// PQF: as in hnsw_walk_flagged, the bitmap of query row q is p.query_filter[q]
+template <int EPL, int CR, int CB, bool SMEM_TABLE, bool PQF>
 __global__ void hnsw_walk_general(const GraphDev g, const SearchParams p, const int has_del, const int table_stride_bytes) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -924,12 +930,16 @@ __global__ void hnsw_walk_general(const GraphDev g, const SearchParams p, const 
   uint32_t *touched = p.touched + slot * (int64_t)p.touched_cap;
   uint64_t *gbag = p.cand + slot * (int64_t)p.cand_cap;
   const uint32_t *filter = p.filter;
-  const bool use_filter = filter != nullptr;
+  bool use_filter = filter != nullptr;
 
   for (;;) {
     const int64_t wi = next_query(p.work_counter, lane);
     if (wi >= p.B) break;
     const int64_t q = p.qmap ? (int64_t)__ldg(p.qmap + wi) : wi;  // subset re-run: outputs stay indexed by query row
+    if constexpr (PQF) {
+      filter = p.query_filter[q];
+      use_filter = filter != nullptr;
+    }
     const float *T;
     if (SMEM_TABLE) {
       __syncwarp();
@@ -1223,7 +1233,7 @@ LaunchGeom pick_geometry(annb_index *h, size_t table_bytes_in, size_t extra_per_
   return best;
 }
 
-template <int EPL, int CR, int CB>
+template <int EPL, int CR, int CB, bool PQF>
 int launch_walk(annb_index *h, const SearchParams &p_in, bool general) {
   SearchParams p = p_in;
   const size_t table_bytes = (size_t)h->M * h->Ks * sizeof(float);
@@ -1283,8 +1293,8 @@ int launch_walk(annb_index *h, const SearchParams &p_in, bool general) {
     }
 #undef ANNB_LAUNCH_FAST
   } else {
-    if (geo.smem_table) ANNB_OCC((hnsw_walk_general<EPL, CR, CB, true>));
-    else ANNB_OCC((hnsw_walk_general<EPL, CR, CB, false>));
+    if (geo.smem_table) ANNB_OCC((hnsw_walk_general<EPL, CR, CB, true, PQF>));
+    else ANNB_OCC((hnsw_walk_general<EPL, CR, CB, false, PQF>));
     int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * occ, (p.B + geo.warps - 1) / geo.warps);
     int64_t slots = (int64_t)blocks * geo.warps;
     p.visited_words = (h->gd.n + 31) / 32;
@@ -1312,9 +1322,9 @@ int launch_walk(annb_index *h, const SearchParams &p_in, bool general) {
       if ((rc = annb_scratch(h, 7, (size_t)slots * p.cand_cap * 8, (void **)&p.cand))) return rc;
       ANNB_CUDA(cudaMemsetAsync(counter, 0, 8, h->stream));
       if (geo.smem_table)
-        hnsw_walk_general<EPL, CR, CB, true><<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, has_del, table_stride);
+        hnsw_walk_general<EPL, CR, CB, true, PQF><<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, has_del, table_stride);
       else
-        hnsw_walk_general<EPL, CR, CB, false><<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, has_del, table_stride);
+        hnsw_walk_general<EPL, CR, CB, false, PQF><<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, has_del, table_stride);
       h->launches++;
       ANNB_CUDA(cudaGetLastError());
       int32_t flag = 0;
@@ -1337,22 +1347,28 @@ int launch_walk(annb_index *h, const SearchParams &p_in, bool general) {
   return ANNB_OK;
 }
 
+template <int EPL, int CR, int CB>
+int launch_walk_q(annb_index *h, const SearchParams &p, bool general) {
+  if (general && p.query_filter) return launch_walk<EPL, CR, CB, true>(h, p, general);
+  return launch_walk<EPL, CR, CB, false>(h, p, general);
+}
+
 template <int EPL>
 int dispatch_code(annb_index *h, const SearchParams &p, bool general) {
   const int cr = h->gd.code_row, cb = h->code_bytes;
   if (cb == 1) {
     switch (cr) {
-      case 4: return launch_walk<EPL, 4, 1>(h, p, general);
-      case 8: return launch_walk<EPL, 8, 1>(h, p, general);
-      case 16: return launch_walk<EPL, 16, 1>(h, p, general);
-      case 32: return launch_walk<EPL, 32, 1>(h, p, general);
-      default: return launch_walk<EPL, 0, 1>(h, p, general);
+      case 4: return launch_walk_q<EPL, 4, 1>(h, p, general);
+      case 8: return launch_walk_q<EPL, 8, 1>(h, p, general);
+      case 16: return launch_walk_q<EPL, 16, 1>(h, p, general);
+      case 32: return launch_walk_q<EPL, 32, 1>(h, p, general);
+      default: return launch_walk_q<EPL, 0, 1>(h, p, general);
     }
   } else {
     switch (cr) {
-      case 8: return launch_walk<EPL, 8, 2>(h, p, general);
-      case 16: return launch_walk<EPL, 16, 2>(h, p, general);
-      default: return launch_walk<EPL, 0, 2>(h, p, general);
+      case 8: return launch_walk_q<EPL, 8, 2>(h, p, general);
+      case 16: return launch_walk_q<EPL, 16, 2>(h, p, general);
+      default: return launch_walk_q<EPL, 0, 2>(h, p, general);
     }
   }
 }
@@ -1366,7 +1382,7 @@ int launch_flagged(annb_index *h, const SearchParams &p_in) {
   int max_warps = 32;
   LaunchGeom geo = pick_geometry(h, table_bytes, extra, max_warps);
   if (!geo.smem_table) return 1;  // not applicable: caller falls back to the bitmap walk
-  auto kern = hnsw_walk_flagged<EPL, CR, CB>;
+  auto kern = p.query_filter ? hnsw_walk_flagged<EPL, CR, CB, true> : hnsw_walk_flagged<EPL, CR, CB, false>;
   int occ = 0, threads = 0, table_stride = (int)((table_bytes + 15) / 16 * 16);
   for (;;) {
     threads = geo.warps * 32;

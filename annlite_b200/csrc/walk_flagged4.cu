@@ -67,7 +67,9 @@ constexpr int w4f_min_ctas(int M, int EP, int EN) {  // register cap = 64K / (ma
   return (tf > tt ? tf : tt) / w4f_max_threads(M, EP, EN);
 }
 
-template <int M, int EP, int EN>
+// PQF (per-query filter): query q is admitted by the bitmap p.query_filter[q] (nullptr = "not deleted") instead of the
+// launch's one p.filter; the choice is made at the start of each query.  PQF = false is the single-filter walk.
+template <int M, int EP, int EN, bool PQF>
 __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP, EN))
     hnsw_walk4f(const GraphDev g, const SearchParams p, const int has_del) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -91,11 +93,11 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
   const int wl = (ef - 1) / EP, ws = (ef - 1) % EP;  // P's position ef-1: lowerBound once P is full
   // admission bit by internal id: the filter bitmap (:353-354, :423-426; delete marks are ignored under a filter),
   // else "not deleted" (:254, :314)
-  const bool use_filter = p.filter != nullptr;
+  bool use_filter = p.filter != nullptr;
   const uint32_t *__restrict__ bits = use_filter ? p.filter : g.deleted;
-  const uint32_t flip = use_filter ? 0u : 1u;
+  uint32_t flip = use_filter ? 0u : 1u;
   auto passes = [&](uint32_t id) -> uint32_t { return ((__ldg(bits + (id >> 5)) >> (id & 31)) & 1u) ^ flip; };
-  const bool size_guard = !use_filter && has_del;  // :270 breaks only when top_candidates is full; :371 has no such guard
+  bool size_guard = !use_filter && has_del;  // :270 breaks only when top_candidates is full; :371 has no such guard
 
   const bool has_slot0 = lane < g.maxM0;
   const uint8_t *link_base0 = g.rec0 + 4 * lane;
@@ -122,6 +124,13 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
     const int64_t q = __reduce_max_sync(FULL_MASK, qi);
     if (q >= p.B) break;
     __syncwarp();
+    if constexpr (PQF) {
+      const uint32_t *f = p.query_filter[q];
+      use_filter = f != nullptr;
+      bits = use_filter ? f : g.deleted;
+      flip = use_filter ? 0u : 1u;
+      size_guard = !use_filter && has_del;
+    }
     if (fused) {
       const float *qg = p.queries + q * (int64_t)(M * p.ds);
       if (p.cb_vec == 4) build_table<M, 4>(T, qg, p.cbt, p.ds, p.is_ip, p.bias, lane);
@@ -373,7 +382,7 @@ template <int M, int EP, int EN>
 int launch_walk4f_t(annb_index *h, const SearchParams &p_in) {
   SearchParams p = p_in;
   static_assert(w4f_fits(M, EP, EN, true) && w4f_fits(M, EP, EN, false), "walk4f geometry exceeds the SM's shared memory");
-  auto kern = hnsw_walk4f<M, EP, EN>;
+  auto kern = p.query_filter ? hnsw_walk4f<M, EP, EN, true> : hnsw_walk4f<M, EP, EN, false>;
   const bool fused = p.queries != nullptr;
   int warps = w4f_cta_warps(M, EP, EN, fused), ctas = w4f_ctas(M, EP, EN, fused);
   if (h->opt_warps_per_cta > 0) warps = (int)std::min<int64_t>(h->opt_warps_per_cta, warps);

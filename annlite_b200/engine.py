@@ -10,6 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib as L
+from .filter import pack_programs
 
 _METRIC = {'l2': L.METRIC_L2, 'euclidean': L.METRIC_L2, 'ip': L.METRIC_IP, 'inner_product': L.METRIC_IP,
            'cosine': L.METRIC_COSINE}
@@ -319,6 +320,51 @@ class Engine:
         L.check(self._lib.annb_filter_prepare(self._h, prog.ctypes.data if prog.size else None, int(prog.shape[0]),
                                               cst.ctypes.data, len(consts), C.byref(fid), C.byref(cnt)))
         return fid.value, cnt.value
+
+    def filter_prepare_many(self, compiled):
+        """compiled: a list of (program, consts) -> (filter ids int32 (F,), admitted counts int64 (F,)), one call."""
+        ops, n_ops, consts, n_const = pack_programs(compiled)
+        F = len(compiled)
+        ids, counts = np.zeros(F, dtype=np.int32), np.zeros(F, dtype=np.int64)
+        cst = consts if len(consts) else np.zeros(8, dtype=np.uint8)
+        L.check(self._lib.annb_filter_prepare_many(self._h, F, ops.ctypes.data if ops.size else None, n_ops.ctypes.data,
+                                                   cst.ctypes.data, n_const.ctypes.data, ids.ctypes.data, counts.ctypes.data))
+        return ids, counts
+
+    def search_multi(self, queries, query_filter, k=10, ef=50, normalize=0, out_labels=None, out_dists=None):
+        """annb_search_multi: query_filter[i] = prepared filter id of query i, 0 = none."""
+        q = self._as_f32(queries)
+        B = q.shape[0]
+        qf = np.ascontiguousarray(query_filter, dtype=np.int32)
+        if qf.shape != (B,):
+            raise ValueError(f'{qf.shape[0] if qf.ndim == 1 else qf.shape} filters for {B} queries')
+        if out_labels is None:
+            out_labels = np.empty((B, k), dtype=np.uint64)
+            out_dists = np.empty((B, k), dtype=np.float32)
+        qp, qs, _k0 = L.as_ptr(q)
+        lp, ls, _k1 = L.as_ptr(out_labels)
+        dp, ds_, _k2 = L.as_ptr(out_dists)
+        assert ls == ds_
+        L.check(self._lib.annb_search_multi(self._h, qp, qs, B, int(normalize), int(k), int(ef), qf.ctypes.data, lp, dp, ls))
+        return out_labels, out_dists
+
+    def search_submit_multi(self, queries, query_filter, out_labels, out_dists, k=10, ef=50, normalize=0):
+        """Streamed form of search_multi: a ticket for search_wait, as search_submit."""
+        q = self._as_f32(queries)
+        qf = np.ascontiguousarray(query_filter, dtype=np.int32)
+        if qf.shape != (q.shape[0],):
+            raise ValueError(f'{qf.shape[0] if qf.ndim == 1 else qf.shape} filters for {q.shape[0]} queries')
+        qp, qs, k0 = L.as_ptr(q)
+        lp, ls, k1 = L.as_ptr(out_labels)
+        dp, ds_, k2 = L.as_ptr(out_dists)
+        assert ls == ds_
+        t = C.c_int()
+        L.check(self._lib.annb_search_submit_multi(self._h, qp, qs, q.shape[0], int(normalize), int(k), int(ef), qf.ctypes.data,
+                                                   lp, dp, ls, C.byref(t)))
+        self._inflight = getattr(self, '_inflight', {})
+        self._inflight[t.value] = (k0, k1, k2, None)
+        self._next_ticket = t.value + 1
+        return t.value
 
     def filter_labels(self, filter_id, count):
         out = np.empty(max(int(count), 1), dtype=np.uint64)

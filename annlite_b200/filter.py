@@ -341,3 +341,18 @@ def compile_filter(where, columns, types, dictionaries):
         walk(tree)
     program = np.array(prog.ops, dtype=L.FILTER_OP)
     return program, bytes(prog.consts)
+
+
+def pack_programs(compiled):
+    """[(program, consts), ...] -> the buffers of annb_filter_prepare_many: all ops back to back (FILTER_OP), n_ops
+    (int32 per program), all constant pools back to back (uint8; each pool keeps its own offsets) and their sizes
+    (int64 per program)."""
+    if len(compiled) > L.FILTER_MAX_PER_CALL:
+        raise ValueError(f'{len(compiled)} distinct filters in one call (limit {L.FILTER_MAX_PER_CALL})')
+    progs = [np.ascontiguousarray(p, dtype=L.FILTER_OP) for p, _ in compiled]
+    pools = [bytes(c) for _, c in compiled]
+    ops = np.concatenate(progs) if progs else np.zeros(0, dtype=L.FILTER_OP)
+    n_ops = np.array([len(p) for p in progs], dtype=np.int32)
+    consts = np.frombuffer(b''.join(pools), dtype=np.uint8).copy()
+    n_const = np.array([len(c) for c in pools], dtype=np.int64)
+    return ops, n_ops, consts, n_const

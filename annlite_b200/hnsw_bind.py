@@ -208,6 +208,25 @@ class Index:
         return self._e.search_prepared(queries, filter_id, k=int(k), ef=self.default_ef, normalize=normalize,
                                        out_labels=out_labels, out_dists=out_dists)
 
+    def knn_query_multi(self, queries, query_filter, k=1, normalize=0, out_labels=None, out_dists=None):
+        """Extension: knn_query_vectors with one prepared filter per query (annb_search_multi); 0 = no filter."""
+        self._need_pq()
+        return self._e.search_multi(queries, query_filter, k=int(k), ef=self.default_ef, normalize=normalize,
+                                    out_labels=out_labels, out_dists=out_dists)
+
+    def knn_query_submit_multi(self, queries, query_filter, k=1, normalize=0, out_labels=None, out_dists=None):
+        """Extension: streamed form of knn_query_multi (annb_search_submit_multi); finish with knn_query_wait."""
+        self._need_pq()
+        B = queries.shape[0]
+        if out_labels is None:
+            out_labels = np.empty((B, int(k)), dtype=np.uint64)
+            out_dists = np.empty((B, int(k)), dtype=np.float32)
+        t = self._e.search_submit_multi(queries, query_filter, out_labels, out_dists, k=int(k), ef=self.default_ef,
+                                        normalize=normalize)
+        self._tickets = getattr(self, '_tickets', {})
+        self._tickets[t] = (out_labels, out_dists)
+        return t
+
     def knn_query_submit(self, queries, k=1, normalize=0, out_labels=None, out_dists=None, filters=None, prepared=None):
         """Extension: streamed form of knn_query_vectors / knn_query_with_filter (annb_search_submit[_filtered]):
         returns a ticket; up to two batches are in flight.  `knn_query_wait(ticket)` returns (labels, dists).

@@ -25,6 +25,13 @@ from .enums import Metric
 logger = logging.getLogger(__name__)
 
 
+def is_per_query_filter(filter):
+    """A list or tuple of filter dicts (None or {} = no filter for that query): one filter per query.  Every other
+    form (a dict, an id array or list, a boolean mask, []) keeps its meaning."""
+    return (isinstance(filter, (list, tuple)) and len(filter) > 0
+            and all(f is None or isinstance(f, dict) for f in filter))
+
+
 class AnnLite:
     def __init__(self, n_dim: int, metric: Union[str, Metric] = 'cosine', n_cells: int = 1,
                  n_subvectors: Optional[int] = None, n_clusters: Optional[int] = 256, n_probe: int = 16,
@@ -184,11 +191,21 @@ class AnnLite:
     # ---- search ---------------------------------------------------------------------------------------
     def search_numpy(self, query_np: 'np.ndarray', filter=None, limit: int = 10, **kwargs):
         """annlite/index.py:485-522: (dists (B, limit), ids (B, limit)); EUCLIDEAN distances are sqrt'ed
-        like HnswIndex.search does.  `filter` = a filter dict over the columns, or the admissible ids."""
+        like HnswIndex.search does.  `filter` = a filter dict over the columns, the admissible ids, or a list of B
+        filter dicts (one per query; None or {} = none): row i is then what query i alone with its filter returns,
+        padded with UINT64_MAX / +inf where its filter admits fewer than `limit` rows."""
         if not self.is_trained:
             raise RuntimeError('The indexer is not trained, cannot add new documents')
         self._sanity_check(query_np)
         indices = None
+        if is_per_query_filter(filter):
+            if len(filter) != query_np.shape[0]:
+                raise ValueError(f'{len(filter)} filters for {query_np.shape[0]} queries')
+            prepared = self._index.prepare_filters(filter)
+            try:
+                return self._index.search_batch(query_np, limit=limit, filter=prepared)
+            finally:
+                prepared.release()
         if filter is not None and not (isinstance(filter, dict) and not filter):
             if isinstance(filter, dict):
                 prepared = self._index.prepare_filter(filter)

@@ -312,6 +312,35 @@ ANNB_API int annb_search_submit_prepared(annb_index_t *h, const float *queries, 
                                 int k, int ef, int filter_id, uint64_t *labels_out, float *dists_out, int out_space,
                                 int *ticket_out);
 
+/* ---- per-query filters ---------------------------------------------------------------------------
+ * A serving batch whose requests carry their own filter (the executor's `filter` per request; CellContainer.search
+ * runs one CellTable.query per call, annlite/container.py:107-120).  annb_filter_prepare_many evaluates F programs in
+ * one pass over the rows: the programs are given back to back (program f = n_ops[f] ops, its pool n_const_bytes[f]
+ * bytes, each pool a multiple of 8 and addressed from its own start); a warp runs all of them over its 32 rows.  Sets
+ * larger than one launch's shared memory (the two LAUNCH limits) are split into several launches inside the call,
+ * which still synchronises once.  Every program is validated as annb_filter_prepare does before anything runs; each
+ * referenced column is synced once; each filter gets its own id (annb_filter_release) and goes stale like one from
+ * annb_filter_prepare. */
+#define ANNB_FILTER_MAX_PER_CALL 1024            /* distinct filters per call (a bitmap is n/8 bytes: 125 KB at 1M rows) */
+#define ANNB_FILTER_LAUNCH_MAX_OPS 2048          /* ops one evaluator launch holds in shared memory                       */
+#define ANNB_FILTER_LAUNCH_MAX_CONST_BYTES 65536 /* constant bytes one evaluator launch holds                             */
+ANNB_API int annb_filter_prepare_many(annb_index_t *h, int F, const annb_filter_op_t *programs, const int *n_ops,
+                             const void *consts, const int64_t *n_const_bytes, int *filter_ids_out, int64_t *counts_out);
+/* knn_query_with_filter (bindings/hnsw_bindings.cpp:393-516) with one filter per query: query_filter[i] is a prepared
+ * filter id, or 0 for no filter (ids start at 1).  Row i is what annb_search_prepared (or annb_search without a filter)
+ * returns for query i alone, in ids and distance bits: the batch is split into unfiltered rows, rows whose filter
+ * suits hnsw_walk4f and the other filtered rows; each group is one launch over its rows gathered into a contiguous
+ * block (hnsw_walk4f's list sized by the group's smallest selectivity), each query reads its own bitmap, queries that
+ * outgrew their list are re-run on the bitmap walk with their own bitmap, and the outputs are scattered back.  Any
+ * query with fewer than k results gives ANNB_EFEWRESULTS (outputs filled, missing slots UINT64_MAX / +inf).
+ * annb_search_submit_multi is the streamed form on the two lanes of annb_search_submit, finished by annb_search_wait
+ * (re-runs happen inside the wait). */
+ANNB_API int annb_search_multi(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
+                      const int *query_filter, uint64_t *labels_out, float *dists_out, int out_space);
+ANNB_API int annb_search_submit_multi(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k,
+                             int ef, const int *query_filter, uint64_t *labels_out, float *dists_out, int out_space,
+                             int *ticket_out);
+
 /* ---- shard merge (CellContainer.ivf_search merge rule, annlite/container.py:130-138) ---------- */
 
 /* G per-shard result lists (G,B,k) (as all-gathered over NCCL) -> (B,k) global top-k by
