@@ -16,6 +16,7 @@ OK, EINVAL, ENODEVICE, ECUDA, ENOMEM, ESTATE, EFEWRESULTS, EIO, ECAPACITY, ENOTF
 HOST, DEVICE = 0, 1
 METRIC_L2, METRIC_IP, METRIC_COSINE = 0, 1, 2
 MAX_EF = 512
+MAX_CELLS, CELLS_GENERIC = 256, 1
 ATTR_INTEGER, ATTR_FLOAT, ATTR_TEXT = 0, 1, 2
 MAX_ATTR_COLUMNS, FILTER_MAX_OPS, FILTER_MAX_DEPTH, FILTER_MAX_CONST_BYTES = 64, 256, 32, 32768
 FILTER_MAX_PER_CALL, FILTER_LAUNCH_MAX_OPS, FILTER_LAUNCH_MAX_CONST_BYTES = 1024, 2048, 65536
@@ -80,6 +81,12 @@ PROTOTYPES = {
     'annb_search_submit_multi': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _vp, _vp, _vp, _int, C.POINTER(_int)]),
     'annb_merge_topk': (_int,[_vp, _vp, _vp, _int, _i64, _int, _vp, _vp]),
     'annb_merge_topk_packed': (_int, [_vp, _vp, _int, _i64, _int, _i64, _i64, _vp, _vp, _int]),
+    'annb_cellset_create': (_int, [_vp, _int, _vp, _int, C.POINTER(_vp)]),
+    'annb_cellset_destroy': (_int, [_vp]),
+    'annb_cellset_search': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp]),
+    'annb_cellset_merge': (_int, [_vp, _vp, _vp, _vp, _vp, _int, _i64, _int, _int, _vp, _vp, _vp, _int]),
+    'annb_cellset_probe': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int]),
+    'annb_cellset_last_ms': (_int, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(_int)]),
     'annb_lane_stream': (_int, [_vp, _int, C.POINTER(_u64)]),
     'annb_last_kernel_ms': (_int, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     'annb_launch_count': (_int, [_vp, C.POINTER(_i64)]),

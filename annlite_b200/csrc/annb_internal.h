@@ -145,6 +145,13 @@ struct SearchParams {
   // per-query filters (annb_search_multi): B bitmaps by internal id, one per query row of this launch (the row qmap
   // names, for the bitmap walk), nullptr = "not deleted"; nullptr here = every query uses `filter`
   const uint32_t *const *query_filter;
+  // multi-cell walk (hnsw_walk4<M, EPL, true>, annb_cellset_search): the device array of the cells' graphs, each
+  // query's probe order (B, n_probe) and each cell's k (0 = skip the cell).  Outputs by cell: row q * n_cells + c of
+  // out_found / out_stats, and cell_limit entries of out_labels / out_dists per row
+  const GraphDev *cells;
+  const int32_t *cell_order;
+  const int32_t *cell_k;
+  int n_cells, n_probe, cell_limit;
 };
 
 // ------------------------------------------------------------------------------------------
@@ -325,6 +332,7 @@ int launch_search(annb_index *h, const SearchParams &p, int mode);
 bool walk4_applicable(const annb_index *h);
 bool walk4_can_fuse(const annb_index *h);
 int launch_walk4(annb_index *h, const SearchParams &p);
+int launch_walk4_cells(annb_index *h, const SearchParams &p);
 // hnsw_walk4f (walk_flagged4.cu): the filtered / deletion-aware search on two register lists, same table handling as
 // hnsw_walk4; returns 1 = not applicable (then hnsw_walk_flagged or the bitmap walk serve the call)
 bool walk4f_applicable(const annb_index *h, int ef, double selectivity);

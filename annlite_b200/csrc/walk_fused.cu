@@ -66,8 +66,12 @@ constexpr int w4_min_ctas(int M, int EPL) {  // register cap = 64K / (max thread
 }
 
 // =====================================================================================================
-template <int M, int EPL>
-__global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) hnsw_walk4(const GraphDev g, const SearchParams p) {
+// CELLS: the multi-cell (IVF) walk of annb_cellset_search.  The work item is a query: its table is built once and then
+// walked over each of its probed cells in probe order (p.cells, p.cell_order; the cells share one PQ codebook), the
+// results of cell c going to row q * n_cells + c of the by-cell scratch.  `g_in` is unused then.  CELLS = false is the
+// single-graph walk.
+template <int M, int EPL, bool CELLS>
+__global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) hnsw_walk4(const GraphDev g_in, const SearchParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
   // warp index through a warp reduction: the compiler then knows it is warp-uniform, keeps the table base in
@@ -84,23 +88,24 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
     if (lane == 0) mbar_init(tbar, 1);
     __syncwarp();
   }
-  const int ef = p.ef;
-  const int k = p.k;
+  // per cell (CELLS): the cell's ef and k; and with them everything below that depends on the graph
+  int ef = p.ef;
+  int k = p.k;
   const bool lane0 = lane == 0;
   const bool stats = p.out_stats != nullptr;
   // list positions ef-1 (lowerBound once full) and ef (the slot an insertion into a full list spills to)
-  const int wl = (ef - 1) / EPL, ws = (ef - 1) % EPL;
+  int wl = (ef - 1) / EPL, ws = (ef - 1) % EPL;
   // per-lane record addressing
-  const bool has_slot0 = lane < g.maxM0;
-  const uint8_t *link_base0 = g.rec0 + 4 * lane;
+  bool has_slot0 = lane < g_in.maxM0;
+  const uint8_t *link_base0 = g_in.rec0 + 4 * lane;
   {  // keep the per-lane base as ONE 64-bit register pair (no re-derivation from the constant bank per load)
     uint64_t t = reinterpret_cast<uint64_t>(link_base0);
     asm volatile("" : "+l"(t));
     link_base0 = reinterpret_cast<const uint8_t *>(t);
   }
-  const unsigned code_delta0 = (unsigned)(g.code_off0 + lane * (M - 4));  // from a lane's link to the same lane's code row
-  const uint32_t rec0_bytes = (uint32_t)g.rec0_bytes;
-  const bool has_slotu = lane < g.maxM;
+  unsigned code_delta0 = (unsigned)(g_in.code_off0 + lane * (M - 4));  // from a lane's link to the same lane's code row
+  uint32_t rec0_bytes = (uint32_t)g_in.rec0_bytes;
+  bool has_slotu = lane < g_in.maxM;
 
   for (;;) {
     // next query: ONE lane bumps the work counter and the value is spread with a warp REDUCTION, not a shuffle:
@@ -136,6 +141,32 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
       float *o = p.dump_tables + q * TS;
       for (int i = lane; i < TS; i += 32) o[i] = T[i];
     }
+
+    for (int ci = 0; ci < (CELLS ? p.n_probe : 1); ci++) {
+    int64_t oq = q;  // output row
+    if constexpr (CELLS) {
+      const int c = __ldg(p.cell_order + q * p.n_probe + ci);
+      k = __ldg(p.cell_k + c);
+      oq = q * p.n_cells + c;
+      if (k == 0) {  // no live rows: the cell is skipped (container.py:104-105)
+        if (lane0) p.out_found[oq] = 0;
+        continue;
+      }
+      const GraphDev &gc = p.cells[c];
+      ef = max(p.ef, k);  // hnswalg.h:1279
+      wl = (ef - 1) / EPL;
+      ws = (ef - 1) % EPL;
+      has_slot0 = lane < gc.maxM0;
+      uint64_t t = reinterpret_cast<uint64_t>(gc.rec0 + 4 * lane);
+      asm volatile("" : "+l"(t));
+      link_base0 = reinterpret_cast<const uint8_t *>(t);
+      code_delta0 = (unsigned)(gc.code_off0 + lane * (M - 4));
+      rec0_bytes = (uint32_t)gc.rec0_bytes;
+      has_slotu = lane < gc.maxM;
+    }
+    const GraphDev &g = CELLS ? p.cells[__ldg(p.cell_order + q * p.n_probe + ci)] : g_in;
+    // outputs start at entry (CELLS ? oq * p.cell_limit : q * k), written out at each use: a hoisted copy reschedules the
+    // single-graph walk
 
     // ---- greedy descent maxlevel..1 (hnswalg.h:1245-1274), walk4_common.cuh ----
     int hops = 0, nbrs = 0, evals = 1;
@@ -297,8 +328,8 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
       const int pos = lane * EPL + e;
       if (pos < k) {
         const bool have = pos < size;
-        p.out_dists[q * k + pos] = have ? u2f(K[e]) : CUDART_INF_F;
-        p.out_labels[q * k + pos] = have ? (p.out_internal ? (uint64_t)(V[e] & IDM) : __ldg(g.labels + (V[e] & IDM))) : (uint64_t)UINT64_MAX;
+        p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? u2f(K[e]) : CUDART_INF_F;
+        p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? (p.out_internal ? (uint64_t)(V[e] & IDM) : __ldg(g.labels + (V[e] & IDM))) : (uint64_t)UINT64_MAX;
       }
       const uint32_t nk = (e + 1 < EPL) ? K[e + 1 < EPL ? e + 1 : e] : k_next_lane;
       tie |= (pos + 1 < found) && (nk == K[e]) && (e + 1 < EPL || lane < 31);
@@ -308,35 +339,36 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
       __syncwarp();
       if (lane0) {
         for (int i = 1; i < found; i++) {
-          const float d = p.out_dists[q * k + i];
-          const uint64_t l = p.out_labels[q * k + i];
+          const float d = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + i];
+          const uint64_t l = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + i];
           int j = i - 1;
-          while (j >= 0 && p.out_dists[q * k + j] == d && p.out_labels[q * k + j] > l) {
-            p.out_dists[q * k + j + 1] = p.out_dists[q * k + j];
-            p.out_labels[q * k + j + 1] = p.out_labels[q * k + j];
+          while (j >= 0 && p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j] == d && p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j] > l) {
+            p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j];
+            p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j];
             j--;
           }
-          p.out_dists[q * k + j + 1] = d;
-          p.out_labels[q * k + j + 1] = l;
+          p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = d;
+          p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = l;
         }
       }
     }
     if (lane0) {
-      p.out_found[q] = found;
+      p.out_found[oq] = found;
       if (stats) {
-        p.out_stats[q * 3 + 0] = hops;
-        p.out_stats[q * 3 + 1] = nbrs;
-        p.out_stats[q * 3 + 2] = evals;
+        p.out_stats[oq * 3 + 0] = hops;
+        p.out_stats[oq * 3 + 1] = nbrs;
+        p.out_stats[oq * 3 + 2] = evals;
       }
+    }
     }
   }
 }
 
-template <int M, int EPL>
+template <int M, int EPL, bool CELLS>
 int launch_walk4_t(annb_index *h, const SearchParams &p_in) {
   SearchParams p = p_in;
   static_assert(w4_fits(M, EPL, true) && w4_fits(M, EPL, false), "walk4 geometry exceeds the SM's shared memory");
-  auto kern = hnsw_walk4<M, EPL>;
+  auto kern = hnsw_walk4<M, EPL, CELLS>;
   const bool fused = p.queries != nullptr;
   int warps = fused ? w4_cta_warps(M, EPL, true) : w4_cta_warps(M, EPL, false);
   int ctas = fused ? w4_ctas(M, EPL, true) : w4_ctas(M, EPL, false);
@@ -366,13 +398,13 @@ int launch_walk4_t(annb_index *h, const SearchParams &p_in) {
   return ANNB_OK;
 }
 
-template <int M>
+template <int M, bool CELLS>
 int launch_walk4_m(annb_index *h, const SearchParams &p) {
   const int epl = (p.ef + 31) / 32;
-  if (epl <= 2) return launch_walk4_t<M, 2>(h, p);
-  if (epl <= 4) return launch_walk4_t<M, 4>(h, p);
-  if (epl <= 8) return launch_walk4_t<M, 8>(h, p);
-  return launch_walk4_t<M, 16>(h, p);
+  if (epl <= 2) return launch_walk4_t<M, 2, CELLS>(h, p);
+  if (epl <= 4) return launch_walk4_t<M, 4, CELLS>(h, p);
+  if (epl <= 8) return launch_walk4_t<M, 8, CELLS>(h, p);
+  return launch_walk4_t<M, 16, CELLS>(h, p);
 }
 
 }  // namespace
@@ -403,9 +435,24 @@ int launch_walk4(annb_index *h, const SearchParams &p) {
   if (!p.queries && (reinterpret_cast<uintptr_t>(p.tables) & 15)) return 1;  // TMA needs 16-byte alignment
   if (p.ef > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "ef=%d exceeds ANNB_MAX_EF=%d", p.ef, ANNB_MAX_EF);
   switch (h->M) {
-    case 8: return launch_walk4_m<8>(h, p);
-    case 16: return launch_walk4_m<16>(h, p);
-    case 32: return launch_walk4_m<32>(h, p);
+    case 8: return launch_walk4_m<8, false>(h, p);
+    case 16: return launch_walk4_m<16, false>(h, p);
+    case 32: return launch_walk4_m<32, false>(h, p);
   }
   return 1;
+}
+
+// The multi-cell walk: p.ef = the caller's ef (cell c walks with max(ef, k_c)), p.cell_limit = the largest k_c; h = the
+// handle whose stream and scratch the launch uses.  Only the fused table build (p.queries) and M = 8 are instantiated: the cell set routes every other
+// geometry to its generic per-cell route.
+int launch_walk4_cells(annb_index *h, const SearchParams &p) {
+  if (p.B == 0) return ANNB_OK;
+  if (!p.queries || h->M != 8) return 1;
+  const int ef_max = std::max(p.ef, p.cell_limit);  // the largest max(ef, k_c) of any cell sizes the list
+  if (ef_max > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, limit)=%d exceeds ANNB_MAX_EF=%d", ef_max, ANNB_MAX_EF);
+  const int epl = (ef_max + 31) / 32;
+  if (epl <= 2) return launch_walk4_t<8, 2, true>(h, p);
+  if (epl <= 4) return launch_walk4_t<8, 4, true>(h, p);
+  if (epl <= 8) return launch_walk4_t<8, 8, true>(h, p);
+  return launch_walk4_t<8, 16, true>(h, p);
 }

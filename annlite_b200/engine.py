@@ -474,3 +474,92 @@ class Engine:
                 x = x.float()
             return x.contiguous()
         return np.ascontiguousarray(np.asarray(x, dtype=np.float32))
+
+
+class CellSet:
+    """annb_cellset_t: multi-cell (IVF) search over the Engines of the cells, which share one PQ codebook.  Borrows
+    them: keep them alive and unmodified during its calls.  `centroids` = the VQ codebook (n_cells, dim) or None."""
+
+    def __init__(self, engines, centroids=None, metric=None):
+        self._lib = L.load()
+        self._h = C.c_void_p()
+        self.engines = list(engines)
+        self.n_cells = len(self.engines)
+        arr = (C.c_void_p * self.n_cells)(*[e._h.value for e in self.engines])
+        cen = None
+        if centroids is not None:
+            cen = np.ascontiguousarray(centroids, dtype=np.float32)
+            if cen.shape != (self.n_cells, self.engines[0].dim):
+                raise ValueError(f'centroids of shape {cen.shape} for {self.n_cells} cells of dim {self.engines[0].dim}')
+        m = self.engines[0].metric if metric is None else metric_code(metric)
+        L.check(self._lib.annb_cellset_create(arr, self.n_cells, cen.ctypes.data if cen is not None else None, int(m),
+                                              C.byref(self._h)))
+
+    def close(self):
+        if getattr(self, '_h', None) is not None and self._h.value:
+            self._lib.annb_cellset_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def search(self, queries, limit=10, ef=50, normalize=0, order=None, n_probe=None, generic=False, with_parts=False):
+        """-> (labels uint64 (B, limit), dists fp32 (B, limit), cells int32 (B, limit)) [+ (part labels, part dists,
+        part counters) (B, n_cells, limit / 3)].  `order` = (B, n_probe) cells per query, or None for the centroids'."""
+        q = Engine._as_f32(queries)
+        B = q.shape[0]
+        if order is not None:
+            order = np.ascontiguousarray(order, dtype=np.int32)
+            n_probe = order.shape[1]
+            if order.shape[0] != B:
+                raise ValueError(f'probe order for {order.shape[0]} queries, got {B}')
+        n_probe = self.n_cells if n_probe is None else int(n_probe)
+        labels = np.empty((B, limit), dtype=np.uint64)
+        dists = np.empty((B, limit), dtype=np.float32)
+        cells = np.empty((B, limit), dtype=np.int32)
+        parts = None
+        if with_parts:
+            parts = (np.empty((B, self.n_cells, limit), dtype=np.uint64), np.empty((B, self.n_cells, limit), dtype=np.float32),
+                     np.empty((B, self.n_cells, 3), dtype=np.int64))
+        qp, qs, _k = L.as_ptr(q)
+        if order is not None and qs == L.DEVICE:
+            raise ValueError('pass the probe order with host queries')
+        L.check(self._lib.annb_cellset_search(
+            self._h, qp, qs, B, int(normalize), order.ctypes.data if order is not None else None, n_probe, int(limit),
+            int(ef), L.CELLS_GENERIC if generic else 0, labels.ctypes.data, dists.ctypes.data, cells.ctypes.data, L.HOST,
+            *([p.ctypes.data for p in parts] if parts else [None, None, None])))
+        return (labels, dists, cells) + ((parts,) if with_parts else ())
+
+    def merge(self, labels, dists, counts, order, limit):
+        """The merge alone over a by-cell scratch (host): labels / dists (B, n_cells, limit), counts (B, n_cells),
+        order (B, n_probe).  -> (labels, dists, cells) (B, limit)."""
+        lab = np.ascontiguousarray(labels, dtype=np.uint64)
+        dis = np.ascontiguousarray(dists, dtype=np.float32)
+        cnt = np.ascontiguousarray(counts, dtype=np.int32)
+        order = np.ascontiguousarray(order, dtype=np.int32)
+        B = order.shape[0]
+        if lab.shape != (B, self.n_cells, limit) or dis.shape != lab.shape or cnt.shape != (B, self.n_cells):
+            raise ValueError('by-cell scratch shapes do not match (B, n_cells, limit)')
+        ol = np.empty((B, limit), dtype=np.uint64)
+        od = np.empty((B, limit), dtype=np.float32)
+        oc = np.empty((B, limit), dtype=np.int32)
+        L.check(self._lib.annb_cellset_merge(self._h, lab.ctypes.data, dis.ctypes.data, cnt.ctypes.data, order.ctypes.data,
+                                             L.HOST, B, order.shape[1], int(limit), ol.ctypes.data, od.ctypes.data,
+                                             oc.ctypes.data, L.HOST))
+        return ol, od, oc
+
+    def probe(self, queries, n_probe=None):
+        q = Engine._as_f32(queries)
+        n_probe = self.n_cells if n_probe is None else int(n_probe)
+        out = np.empty((q.shape[0], n_probe), dtype=np.int32)
+        qp, qs, _k = L.as_ptr(q)
+        L.check(self._lib.annb_cellset_probe(self._h, qp, qs, q.shape[0], n_probe, out.ctypes.data, L.HOST))
+        return out
+
+    def last_ms(self):
+        a, b, c, r = C.c_float(), C.c_float(), C.c_float(), C.c_int()
+        L.check(self._lib.annb_cellset_last_ms(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(r)))
+        return dict(probe_ms=a.value, walk_ms=b.value, merge_ms=c.value, route='fused' if r.value == 0 else 'generic')

@@ -359,6 +359,51 @@ ANNB_API int annb_merge_topk_packed(annb_index_t *h, const void *packed_gathered
                            float *dists_out, int lane);
 ANNB_API int annb_lane_stream(annb_index_t *h, int lane, uint64_t *stream_out);
 
+/* ---- cell sets: multi-cell (IVF) search ---------------------------------------------------------
+ * CellContainer.ivf_search (annlite/container.py:88-144) over n_cells existing handles, one HNSW graph per cell, all
+ * sharing one PQ codebook.  annb_cellset_create rejects handles on different devices, with a different metric or PQ
+ * geometry, or whose codebooks differ, and more than ANNB_MAX_CELLS cells.  `centroids` = the VQ codebook (n_cells,
+ * dim) fp32 host (VQCodec.codebook) or NULL; with it, searches without an explicit order probe cells in the order of
+ * AnnLite._cell_selection (annlite/index.py:458-466): annlite.math.cdist for the metric, ascending, ties by cell.  The
+ * reference's cdist has no inner-product entry, so an IP cell set with centroids is refused (ANNB_EINVAL).  The cell
+ * set borrows the handles: they must outlive it and must not be modified during one of its calls.
+ *
+ * annb_cellset_search: queries (B, dim) host or device (in_space), normalised `normalize` times for the walk (the
+ * probe reads them raw); order = (B, n_probe) int32 cells (in_space) or NULL for the centroid order; every cell's
+ * device graph is brought up to date first.  Cell c is searched with k_c = min(limit, its live rows) (skipped when 0)
+ * and ef_c = max(ef, k_c).  Without deletions, for M = 8 / 256 u8 codes, one launch builds each query's ADC table once
+ * and walks all its probed cells (hnsw_walk4's multi-cell form); otherwise -- or with flags & ANNB_CELLS_GENERIC --
+ * one annb_search per probed cell.  Both then run the merge of annb_cellset_merge (EUCLIDEAN distances sqrt'ed first,
+ * as HnswIndex.search returns them).  Outputs (B, limit): labels, distances, cell of each result; fewer than `limit`
+ * results -> UINT64_MAX / +inf / -1.  part_* (optional, out_space): the by-cell scratch (B, n_cells, limit) labels and
+ * raw distances, and (B, n_cells, 3) counters as annb_search's stats_out; cells a query does not probe are empty.
+ *
+ * annb_cellset_merge: the merge alone over a caller-filled by-cell scratch (in_space): labels / dists (B, n_cells,
+ * limit) as the per-cell searches return them (sqrt'ed for EUCLIDEAN), counts (B, n_cells) entries per row (a row also
+ * ends at its first UINT64_MAX), order (B, n_probe).  In probe order a cell with no results is skipped, and a cell is
+ * dropped when the results so far number >= limit and its nearest distance is greater than the last appended cell's
+ * largest (container.py:122-123); the kept lists are concatenated and the `limit` smallest returned by (distance,
+ * concatenation position), a stable form of container.py:135. */
+#define ANNB_MAX_CELLS 256
+#define ANNB_CELLS_GENERIC 1 /* annb_cellset_search flag: take the per-cell route even where the fused walk applies */
+typedef struct annb_cellset annb_cellset_t;
+ANNB_API int annb_cellset_create(annb_index_t *const *handles, int n_cells, const float *centroids, int metric,
+                        annb_cellset_t **out);
+ANNB_API int annb_cellset_destroy(annb_cellset_t *cs);
+ANNB_API int annb_cellset_search(annb_cellset_t *cs, const float *queries, int in_space, int64_t B, int normalize,
+                        const int32_t *order, int n_probe, int limit, int ef, int flags, uint64_t *labels_out,
+                        float *dists_out, int32_t *cells_out, int out_space, uint64_t *part_labels, float *part_dists,
+                        int64_t *part_stats);
+ANNB_API int annb_cellset_merge(annb_cellset_t *cs, const uint64_t *labels, const float *dists, const int32_t *counts,
+                       const int32_t *order, int in_space, int64_t B, int n_probe, int limit, uint64_t *labels_out,
+                       float *dists_out, int32_t *cells_out, int out_space);
+/* The probe order alone: (B, n_probe) int32 cells per query, nearest centroid first. */
+ANNB_API int annb_cellset_probe(annb_cellset_t *cs, const float *queries, int in_space, int64_t B, int n_probe,
+                       int32_t *order_out, int out_space);
+/* Device time of the last probe / walk (fused launch, or the per-cell searches) / merge in ms, and the route the last
+ * annb_cellset_search took (0 = fused walk, 1 = per-cell searches). */
+ANNB_API int annb_cellset_last_ms(annb_cellset_t *cs, float *probe_ms, float *walk_ms, float *merge_ms, int *route);
+
 /* ---- introspection for bench / roofline ------------------------------------------------------ */
 /* Device time of the last search / scan / table kernel in milliseconds (CUDA events on the
  * handle's stream) and launch counters since creation. */
