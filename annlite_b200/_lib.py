@@ -74,6 +74,7 @@ PROTOTYPES = {
     'annb_filter_prepare': (_int, [_vp, _vp, _int, _vp, _i64, C.POINTER(_int), C.POINTER(_i64)]),
     'annb_filter_labels': (_int, [_vp, _int, _vp, _i64, C.POINTER(_i64)]),
     'annb_filter_release': (_int, [_vp, _int]),
+    'annb_filter_prepare_labels': (_int, [_vp, _vp, _i64, _int, C.POINTER(_int), C.POINTER(_i64)]),
     'annb_search_prepared': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _int, _vp, _vp, _int]),
     'annb_search_submit_prepared': (_int, [_vp, _vp, _int, _i64, _int, _int, _int, _int, _vp, _vp, _int, C.POINTER(_int)]),
     'annb_filter_prepare_many': (_int, [_vp, _int, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -84,6 +85,9 @@ PROTOTYPES = {
     'annb_cellset_create': (_int, [_vp, _int, _vp, _int, C.POINTER(_vp)]),
     'annb_cellset_destroy': (_int, [_vp]),
     'annb_cellset_search': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp]),
+    'annb_cellset_search_prepared': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _int,
+                                            _vp, _vp, _vp]),
+    'annb_cellset_last_filtered': (_int, [_vp, C.POINTER(_i64), C.POINTER(_int)]),
     'annb_cellset_merge': (_int, [_vp, _vp, _vp, _vp, _vp, _int, _i64, _int, _int, _vp, _vp, _vp, _int]),
     'annb_cellset_probe': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int]),
     'annb_cellset_last_ms': (_int, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(_int)]),

@@ -5,7 +5,10 @@ Differences from the reference, besides the docarray / SQLite / RocksDB stores i
 * labels are the caller's ids, unique across cells (the single-cell convention of AnnLite.index); a host label -> cell
   map stands in for the MetaTable.  Results carry those labels, not doc ids looked up per cell offset.
 * a batch of queries runs as one GPU search (annb_cellset_search): without a filter or deletions, one launch builds
-  each query's ADC table once and walks all its probed cells; every other case searches the cells one by one.
+  each query's ADC table once and walks all its probed cells.  A dict filter or an id array is prepared on each probed
+  cell and searched the same way with each cell's bitmap (annb_cellset_search_prepared), deletions included.  Per-query
+  filter lists, cells with `bruteforce_filter_below` set and unfiltered searches after deletions search the cells one
+  by one.
 * equal distances in the merge keep concatenation order (the reference's argsort leaves them unspecified); a query
   with fewer than `limit` results is padded with +inf / UINT64_MAX / cell -1.
 * with a VQCodec attached, cells are probed in the order of annlite.math.cdist over the centroids.  The reference's
@@ -93,10 +96,12 @@ class CellContainer:
         return self._cellset
 
     # ---- insert / update / delete (container.py:262-414) ---------------------------------------------------
-    def insert(self, data: 'np.ndarray', cells: 'np.ndarray', ids=None, tags=None):
+    def insert(self, data: 'np.ndarray', cells: 'np.ndarray', ids=None, tags=None, num_threads: int = -1):
         """Add rows to the given cells.  `ids` = their labels (default: after the largest one so far); a label that
         is already stored is updated: in place when it stays in its cell, else deleted there and inserted into the new
-        cell (container.py:323-386).  `tags` = per-row attribute dicts or a dict of column -> values."""
+        cell (container.py:323-386).  `tags` = per-row attribute dicts or a dict of column -> values.  `num_threads`
+        as in HnswIndex.add_with_ids: 1 = the single-threaded build, whose graphs are the same on every run; any other
+        value inserts in parallel, in an order that varies from run to run."""
         data = np.ascontiguousarray(data, dtype=np.float32)
         cells = np.asarray(cells, dtype=np.int64).reshape(-1)
         n = data.shape[0]
@@ -123,7 +128,8 @@ class CellContainer:
             if tags is not None and idx.attributes.names:
                 rows = [tags[i] for i in sel] if not isinstance(tags, dict) else {k: [v[i] for i in sel] for k, v in tags.items()}
                 attrs = idx.attributes.convert(rows, len(sel))
-            idx.add_with_ids(data[sel], ids[sel])
+            # (the default call is the plain add_with_ids(x, ids): any cell index with that interface works)
+            idx.add_with_ids(data[sel], ids[sel], **({} if num_threads == -1 else {'num_threads': num_threads}))
             if attrs is not None:
                 idx.set_attributes(ids[sel], attrs)
             for label in ids[sel].tolist():
@@ -131,8 +137,8 @@ class CellContainer:
                     self._live[c] += 1
                 self._label_cell[label] = c
 
-    def update(self, data: 'np.ndarray', cells: 'np.ndarray', ids, tags=None):
-        self.insert(data, cells, ids=ids, tags=tags)
+    def update(self, data: 'np.ndarray', cells: 'np.ndarray', ids, tags=None, num_threads: int = -1):
+        self.insert(data, cells, ids=ids, tags=tags, num_threads=num_threads)
 
     def delete(self, ids):
         for label in np.asarray(ids, dtype=np.int64).reshape(-1).tolist():
@@ -175,8 +181,11 @@ class CellContainer:
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
                                        generic=generic)
             return dist, lab, cid
-        # filtered: one filtered search per probed cell (HnswIndex.search_batch shrinks the limit to what the filter
-        # admits there, hnsw/index.py:151-154), then the same merge on the GPU
+        if (not generic and not is_per_query_filter(filter)
+                and all(v.bruteforce_filter_below is None for v in self._vec_indexes)):
+            return self._search_cells_prepared(x, cells, filter, limit)
+        # filtered, per-cell route: one filtered search per probed cell (HnswIndex.search_batch shrinks the limit to
+        # what the filter admits there, hnsw/index.py:151-154), then the same merge on the GPU
         lab = np.full((B, self.n_cells, limit), _NONE, dtype=np.uint64)
         dist = np.full((B, self.n_cells, limit), np.inf, dtype=np.float32)
         counts = np.zeros((B, self.n_cells), dtype=np.int32)
@@ -212,6 +221,40 @@ class CellContainer:
             lab[:, c, :w], dist[:, c, :w], counts[:, c] = i, d, w
         ol, od, oc = cs.merge(lab, dist, counts, cells, limit)
         return od, ol, oc
+
+    def _search_cells_prepared(self, x, cells, filter, limit):
+        """A dict filter or an id array over the probed cells in one GPU search (annb_cellset_search_prepared): the
+        filter is prepared on each probed cell (an id array split by cell, each share prepared as a label list), and
+        every cell's k is what the per-cell route's search_batch uses: min(limit, live rows, admitted count)."""
+        from .core.index.hnsw.index import PreparedFilter
+        cs = self._cells()
+        v0 = self._vec_indexes[0]
+        fids = np.zeros(self.n_cells, dtype=np.int32)
+        prepared = []
+        if not isinstance(filter, dict):
+            allowed = np.asarray(filter)
+            allowed = (np.nonzero(allowed)[0] if allowed.dtype == bool else allowed).astype(np.int64)
+            cell_of = np.array([self._label_cell.get(a, -1) for a in allowed.tolist()], dtype=np.int64)
+        try:
+            for c in np.unique(cells).tolist():
+                if self._live[c] == 0:
+                    continue
+                idx = self._vec_indexes[c]
+                if isinstance(filter, dict):
+                    prepared.append(idx.prepare_filter(filter))
+                else:
+                    mine = allowed[cell_of == c]   # repeats count, as in the per-cell route's len(indices)
+                    if len(mine) == 0:
+                        continue
+                    e = idx._index._e
+                    prepared.append(PreparedFilter(e, *e.filter_prepare_labels(mine.astype(np.uint64))))
+                fids[c] = prepared[-1].id
+            lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
+                                       filter_ids=fids)
+        finally:
+            for p in prepared:
+                p.release()
+        return dist, lab, cid
 
     def filter_cells(self, cells, filter=None, limit: int = -1, offset: int = 0, order_by: Optional[str] = None,
                      ascending: bool = True):

@@ -152,6 +152,9 @@ struct SearchParams {
   const int32_t *cell_order;
   const int32_t *cell_k;
   int n_cells, n_probe, cell_limit;
+  // filtered multi-cell walk (hnsw_walk4f<8, EP, EN, false, true>, annb_cellset_search_prepared): the device array of
+  // the cells' prepared bitmaps by internal id, one per cell
+  const uint32_t *const *cell_filter;
 };
 
 // ------------------------------------------------------------------------------------------
@@ -336,7 +339,16 @@ int launch_walk4_cells(annb_index *h, const SearchParams &p);
 // hnsw_walk4f (walk_flagged4.cu): the filtered / deletion-aware search on two register lists, same table handling as
 // hnsw_walk4; returns 1 = not applicable (then hnsw_walk_flagged or the bitmap walk serve the call)
 bool walk4f_applicable(const annb_index *h, int ef, double selectivity);
+// ... and its list geometry for that search: (ep, en) = entries per lane of P and N; false = not applicable
+bool walk4f_geometry(const annb_index *h, int ef, double selectivity, int *ep_out, int *en_out);
 int launch_walk4f(annb_index *h, const SearchParams &p);
+// the filtered multi-cell walk with lists of (ep, en) entries per lane; returns 1 = not instantiated for these
+int launch_walk4f_cells(annb_index *h, const SearchParams &p, int ep, int en);
+// capi.cu: a live prepared filter of the handle (ANNB_EINVAL unknown, ANNB_ESTATE stale; the caller holds the lock),
+// and annb_search_prepared with annb_search's (B, 3) counters (takes the lock)
+int find_prepared_filter(annb_index *h, int filter_id, PreparedFilter **out);
+int search_prepared_stats(annb_index *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef, int filter_id,
+                          uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out);
 // G ascending (dist, label) lists of k per query -> global k best; *_gstride = distance between two shards' arrays in elements
 int launch_merge_topk(annb_index *h, const uint64_t *labels, const float *dists, int G, int64_t B, int k, int64_t l_gstride,
                       int64_t d_gstride, uint64_t *labels_out, float *dists_out, cudaStream_t stream);

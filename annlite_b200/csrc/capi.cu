@@ -1036,6 +1036,36 @@ int annb_search(annb_index_t *h, const float *queries, const float *tables, int 
 
 }  // extern "C"
 
+// a label list -> the by-id bitmap of the rows it names ((gd.n + 31) / 32 + 1 words), on the handle's stream
+static int labels_to_bitmap(annb_index *h, const uint64_t *filter_labels, int filter_space, int64_t n_filter, uint32_t *by_id) {
+  if (h->max_label > (uint64_t)h->gd.n * 64 + (1ull << 30)) {
+    // labels too sparse for a by-label bitmap on the device: resolve them through the host's
+    // label -> internal id map (the same map mark_deleted uses) and upload the by-id bitmap
+    std::vector<uint64_t> tmp;
+    const uint64_t *hl = filter_labels;
+    if (filter_space == ANNB_DEVICE) {
+      tmp.resize((size_t)n_filter);
+      ANNB_CUDA(cudaMemcpyAsync(tmp.data(), filter_labels, (size_t)n_filter * 8, cudaMemcpyDeviceToHost, h->stream));
+      ANNB_CUDA(cudaStreamSynchronize(h->stream));
+      hl = tmp.data();
+    }
+    std::vector<uint32_t> bm((size_t)(h->gd.n + 31) / 32 + 1, 0u);
+    for (int64_t i = 0; i < n_filter; i++) {
+      auto it = h->g.label_lookup.find(hl[i]);
+      if (it != h->g.label_lookup.end()) bm[it->second >> 5] |= 1u << (it->second & 31);
+    }
+    ANNB_CUDA(cudaMemcpyAsync(by_id, bm.data(), bm.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  } else {
+    const uint64_t *dfl;
+    ANNB_TRY(stage_in(h, filter_labels, filter_space, (size_t)std::max<int64_t>(n_filter, 1) * 8, S_FLT_LABELS, (const void **)&dfl));
+    uint32_t *by_label;
+    ANNB_TRY(annb_scratch(h, S_FLT_BY_LABEL, ((size_t)(h->max_label >> 5) + 1) * 4, (void **)&by_label));
+    ANNB_TRY(launch_filter_bitmap(h, dfl, n_filter, by_label, by_id));
+  }
+  return ANNB_OK;
+}
+
 static int search_impl(annb_index *h, const float *queries, const float *tables, int in_space, int64_t B, int normalize,
                        int k, int ef, const uint64_t *filter_labels, int filter_space, int64_t n_filter,
                        const PreparedFilter *pf, uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out) {
@@ -1162,31 +1192,7 @@ static int search_impl(annb_index *h, const float *queries, const float *tables,
   } else if (filter_labels) {
     uint32_t *by_id;
     ANNB_TRY(annb_scratch(h, S_FLT_BY_ID, ((size_t)(h->gd.n + 31) / 32 + 1) * 4, (void **)&by_id));
-    if (h->max_label > (uint64_t)h->gd.n * 64 + (1ull << 30)) {
-      // labels too sparse for a by-label bitmap on the device: resolve them through the host's
-      // label -> internal id map (the same map mark_deleted uses) and upload the by-id bitmap
-      std::vector<uint64_t> tmp;
-      const uint64_t *hl = filter_labels;
-      if (filter_space == ANNB_DEVICE) {
-        tmp.resize((size_t)n_filter);
-        ANNB_CUDA(cudaMemcpyAsync(tmp.data(), filter_labels, (size_t)n_filter * 8, cudaMemcpyDeviceToHost, h->stream));
-        ANNB_CUDA(cudaStreamSynchronize(h->stream));
-        hl = tmp.data();
-      }
-      std::vector<uint32_t> bm((size_t)(h->gd.n + 31) / 32 + 1, 0u);
-      for (int64_t i = 0; i < n_filter; i++) {
-        auto it = h->g.label_lookup.find(hl[i]);
-        if (it != h->g.label_lookup.end()) bm[it->second >> 5] |= 1u << (it->second & 31);
-      }
-      ANNB_CUDA(cudaMemcpyAsync(by_id, bm.data(), bm.size() * 4, cudaMemcpyHostToDevice, h->stream));
-      ANNB_CUDA(cudaStreamSynchronize(h->stream));
-    } else {
-      const uint64_t *dfl;
-      ANNB_TRY(stage_in(h, filter_labels, filter_space, (size_t)std::max<int64_t>(n_filter, 1) * 8, S_FLT_LABELS, (const void **)&dfl));
-      uint32_t *by_label;
-      ANNB_TRY(annb_scratch(h, S_FLT_BY_LABEL, ((size_t)(h->max_label >> 5) + 1) * 4, (void **)&by_label));
-      ANNB_TRY(launch_filter_bitmap(h, dfl, n_filter, by_label, by_id));
-    }
+    ANNB_TRY(labels_to_bitmap(h, filter_labels, filter_space, n_filter, by_id));
     dfilter = by_id;
   }
   SearchParams p;
@@ -1878,6 +1884,20 @@ static int prepare_many_impl(annb_index *h, int F, const annb_filter_op_t *progr
   return ANNB_OK;
 }
 
+// the cell sets (cells.cu) use a cell's prepared filters under that cell's lock
+int find_prepared_filter(annb_index *h, int filter_id, PreparedFilter **out) { return find_filter(h, filter_id, out); }
+
+// annb_search_prepared with the (B, 3) counters of annb_search; takes the handle's lock
+int search_prepared_stats(annb_index *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef, int filter_id,
+                          uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  PreparedFilter *f;
+  ANNB_TRY(find_filter(h, filter_id, &f));
+  return search_impl(h, queries, nullptr, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, f, labels_out, dists_out, out_space,
+                     stats_out);
+}
+
 extern "C" {
 
 int annb_attr_define(annb_index_t *h, int col, int type) {
@@ -1997,6 +2017,37 @@ int annb_filter_prepare_many(annb_index_t *h, int F, const annb_filter_op_t *pro
     counts_out[f] = 0;
   }
   return prepare_many_impl(h, F, programs, n_ops, consts, n_const_bytes, filter_ids_out, counts_out);
+}
+
+int annb_filter_prepare_labels(annb_index_t *h, const uint64_t *labels, int64_t n, int space, int *filter_id, int64_t *count) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  if (!filter_id || !count || n < 0 || (n > 0 && !labels)) ANNB_FAIL(ANNB_EINVAL, "bad arguments");
+  *filter_id = 0;
+  *count = 0;
+  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
+  ANNB_TRY(drain_lanes(h));  // the label staging buffers are lane 0's
+  ANNB_TRY(sync_device_graph(h));
+  const int64_t rows = h->gd.n;
+  const size_t words = (size_t)(rows + 31) / 32 + 1;
+  void *block = nullptr;
+  ANNB_CUDA(cudaMalloc(&block, words * 4));
+  std::shared_ptr<void> owner(block, [](void *p) { cudaFree(p); });
+  uint32_t *bits = (uint32_t *)block;
+  ANNB_CUDA(cudaMemsetAsync(bits, 0, words * 4, h->stream));
+  ANNB_TRY(labels_to_bitmap(h, labels, space, n, bits));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  PreparedFilter pf;
+  pf.bits = bits;
+  pf.block = owner;
+  pf.n = rows;
+  pf.count = n;  // as a label list counts: every entry, repeats and labels not in the graph included
+  pf.gen = h->state_gen;
+  const int id = h->next_filter_id++;
+  h->filters[id] = pf;
+  *filter_id = id;
+  *count = n;
+  return ANNB_OK;
 }
 
 int annb_filter_labels(annb_index_t *h, int filter_id, uint64_t *labels_out, int64_t cap, int64_t *n_out) {

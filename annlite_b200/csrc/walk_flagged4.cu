@@ -69,9 +69,16 @@ constexpr int w4f_min_ctas(int M, int EP, int EN) {  // register cap = 64K / (ma
 
 // PQF (per-query filter): query q is admitted by the bitmap p.query_filter[q] (nullptr = "not deleted") instead of the
 // launch's one p.filter; the choice is made at the start of each query.  PQF = false is the single-filter walk.
-template <int M, int EP, int EN, bool PQF>
+//
+// CELLS: the filtered multi-cell (IVF) walk of annb_cellset_search_prepared, hnsw_walk4<M, EPL, true>'s work mapping.
+// The work item is a query: its table is built once and then walked over each of its probed cells in probe order
+// (p.cells, p.cell_order), cell c admitting by its own prepared bitmap p.cell_filter[c] (filter semantics in every cell:
+// no size guard) with k_c = p.cell_k[c] (0 = skip the cell) and ef_c = max(ef, k_c).  Results, found and counters go to
+// row q * n_cells + c of the by-cell scratch; a (query, cell) walk that outgrows N writes found = -1 for that pair only
+// and the query goes on with its next cell.  `g_in` and `has_del` are unused then.
+template <int M, int EP, int EN, bool PQF, bool CELLS>
 __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP, EN))
-    hnsw_walk4f(const GraphDev g, const SearchParams p, const int has_del) {
+    hnsw_walk4f(const GraphDev g_in, const SearchParams p, const int has_del) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp = (int)__reduce_min_sync(FULL_MASK, threadIdx.x >> 5);  // uniform register (see hnsw_walk4)
@@ -86,29 +93,35 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
     if (lane == 0) mbar_init(tbar, 1);
     __syncwarp();
   }
-  const int ef = p.ef;
-  const int k = p.k;
+  // per cell (CELLS): the cell's ef and k; and with them everything below that depends on the graph
+  int ef = p.ef;
+  int k = p.k;
   const bool lane0 = lane == 0;
   const bool stats = p.out_stats != nullptr;
-  const int wl = (ef - 1) / EP, ws = (ef - 1) % EP;  // P's position ef-1: lowerBound once P is full
+  int wl = (ef - 1) / EP, ws = (ef - 1) % EP;  // P's position ef-1: lowerBound once P is full
   // admission bit by internal id: the filter bitmap (:353-354, :423-426; delete marks are ignored under a filter),
   // else "not deleted" (:254, :314)
   bool use_filter = p.filter != nullptr;
-  const uint32_t *__restrict__ bits = use_filter ? p.filter : g.deleted;
+  const uint32_t *__restrict__ bits = use_filter ? p.filter : g_in.deleted;
   uint32_t flip = use_filter ? 0u : 1u;
   auto passes = [&](uint32_t id) -> uint32_t { return ((__ldg(bits + (id >> 5)) >> (id & 31)) & 1u) ^ flip; };
   bool size_guard = !use_filter && has_del;  // :270 breaks only when top_candidates is full; :371 has no such guard
+  if constexpr (CELLS) {  // every cell admits by its own bitmap (set per cell below)
+    use_filter = true;
+    flip = 0u;
+    size_guard = false;
+  }
 
-  const bool has_slot0 = lane < g.maxM0;
-  const uint8_t *link_base0 = g.rec0 + 4 * lane;
+  bool has_slot0 = lane < g_in.maxM0;
+  const uint8_t *link_base0 = g_in.rec0 + 4 * lane;
   {
     uint64_t t = reinterpret_cast<uint64_t>(link_base0);
     asm volatile("" : "+l"(t));
     link_base0 = reinterpret_cast<const uint8_t *>(t);
   }
-  const unsigned code_delta0 = (unsigned)(g.code_off0 + lane * (M - 4));
-  const uint32_t rec0_bytes = (uint32_t)g.rec0_bytes;
-  const bool has_slotu = lane < g.maxM;
+  unsigned code_delta0 = (unsigned)(g_in.code_off0 + lane * (M - 4));
+  uint32_t rec0_bytes = (uint32_t)g_in.rec0_bytes;
+  bool has_slotu = lane < g_in.maxM;
 
   for (;;) {
     unsigned qi = 0;
@@ -127,7 +140,7 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
     if constexpr (PQF) {
       const uint32_t *f = p.query_filter[q];
       use_filter = f != nullptr;
-      bits = use_filter ? f : g.deleted;
+      bits = use_filter ? f : g_in.deleted;
       flip = use_filter ? 0u : 1u;
       size_guard = !use_filter && has_del;
     }
@@ -147,6 +160,32 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       float *o = p.dump_tables + q * TS;
       for (int i = lane; i < TS; i += 32) o[i] = T[i];
     }
+
+    for (int ci = 0; ci < (CELLS ? p.n_probe : 1); ci++) {
+    int64_t oq = q;  // output row
+    if constexpr (CELLS) {
+      const int c = __ldg(p.cell_order + q * p.n_probe + ci);
+      k = __ldg(p.cell_k + c);
+      oq = q * p.n_cells + c;
+      if (k == 0) {  // nothing admitted: the cell is skipped
+        if (lane0) p.out_found[oq] = 0;
+        continue;
+      }
+      const GraphDev &gc = p.cells[c];
+      ef = max(p.ef, k);  // hnswalg.h:1279
+      wl = (ef - 1) / EP;
+      ws = (ef - 1) % EP;
+      bits = p.cell_filter[c];
+      has_slot0 = lane < gc.maxM0;
+      uint64_t t = reinterpret_cast<uint64_t>(gc.rec0 + 4 * lane);
+      asm volatile("" : "+l"(t));
+      link_base0 = reinterpret_cast<const uint8_t *>(t);
+      code_delta0 = (unsigned)(gc.code_off0 + lane * (M - 4));
+      rec0_bytes = (uint32_t)gc.rec0_bytes;
+      has_slotu = lane < gc.maxM;
+    }
+    const GraphDev &g = CELLS ? p.cells[__ldg(p.cell_order + q * p.n_probe + ci)] : g_in;
+    // outputs start at entry (CELLS ? oq * p.cell_limit : q * k), written out at each use as in hnsw_walk4
 
     int hops = 0, nbrs = 0, evals = 1;
     uint32_t cur_uk, rec;
@@ -328,7 +367,7 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
     }
 
     if (aborted) {
-      if (lane0) p.out_found[q] = -1;
+      if (lane0) p.out_found[oq] = -1;
       continue;
     }
     // ---- results: the first k admitted entries, ascending (dist, label) (hnsw_bindings.cpp:346-351) ----
@@ -340,49 +379,52 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       const int pos = lane * EP + e;
       if (pos < k) {
         const bool have = pos < found;
-        p.out_dists[q * k + pos] = have ? u2f(KP[e]) : CUDART_INF_F;
-        p.out_labels[q * k + pos] = have ? (p.out_internal ? (uint64_t)(VP[e] & IDM) : __ldg(g.labels + (VP[e] & IDM))) : (uint64_t)UINT64_MAX;
+        p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? u2f(KP[e]) : CUDART_INF_F;
+        p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? (p.out_internal ? (uint64_t)(VP[e] & IDM) : __ldg(g.labels + (VP[e] & IDM))) : (uint64_t)UINT64_MAX;
       }
       const uint32_t nk = (e + 1 < EP) ? KP[e + 1 < EP ? e + 1 : e] : k_next_lane;
       tie |= (pos + 1 < found) && (nk == KP[e]) && (e + 1 < EP || lane < 31);
     }
     for (int r = CAPP + lane; r < k; r += 32) {  // k > 32*EP cannot happen (ef >= k, CAPP >= ef); kept for safety
-      p.out_dists[q * k + r] = CUDART_INF_F;
-      p.out_labels[q * k + r] = (uint64_t)UINT64_MAX;
+      p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + r] = CUDART_INF_F;
+      p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + r] = (uint64_t)UINT64_MAX;
     }
     if (__any_sync(FULL_MASK, tie)) {
       __syncwarp();
       if (lane0) {
         for (int i = 1; i < found; i++) {
-          const float d = p.out_dists[q * k + i];
-          const uint64_t l = p.out_labels[q * k + i];
+          const float d = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + i];
+          const uint64_t l = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + i];
           int j = i - 1;
-          while (j >= 0 && p.out_dists[q * k + j] == d && p.out_labels[q * k + j] > l) {
-            p.out_dists[q * k + j + 1] = p.out_dists[q * k + j];
-            p.out_labels[q * k + j + 1] = p.out_labels[q * k + j];
+          while (j >= 0 && p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j] == d && p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j] > l) {
+            p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j];
+            p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j];
             j--;
           }
-          p.out_dists[q * k + j + 1] = d;
-          p.out_labels[q * k + j + 1] = l;
+          p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = d;
+          p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = l;
         }
       }
     }
     if (lane0) {
-      p.out_found[q] = found;
+      p.out_found[oq] = found;
       if (stats) {
-        p.out_stats[q * 3 + 0] = hops;
-        p.out_stats[q * 3 + 1] = nbrs;
-        p.out_stats[q * 3 + 2] = evals;
+        p.out_stats[oq * 3 + 0] = hops;
+        p.out_stats[oq * 3 + 1] = nbrs;
+        p.out_stats[oq * 3 + 2] = evals;
       }
+    }
     }
   }
 }
 
-template <int M, int EP, int EN>
+template <int M, int EP, int EN, bool CELLS = false>
 int launch_walk4f_t(annb_index *h, const SearchParams &p_in) {
   SearchParams p = p_in;
   static_assert(w4f_fits(M, EP, EN, true) && w4f_fits(M, EP, EN, false), "walk4f geometry exceeds the SM's shared memory");
-  auto kern = p.query_filter ? hnsw_walk4f<M, EP, EN, true> : hnsw_walk4f<M, EP, EN, false>;
+  void (*kern)(const GraphDev, const SearchParams, const int);
+  if constexpr (CELLS) kern = hnsw_walk4f<M, EP, EN, false, true>;
+  else kern = p.query_filter ? hnsw_walk4f<M, EP, EN, true, false> : hnsw_walk4f<M, EP, EN, false, false>;
   const bool fused = p.queries != nullptr;
   int warps = w4f_cta_warps(M, EP, EN, fused), ctas = w4f_ctas(M, EP, EN, fused);
   if (h->opt_warps_per_cta > 0) warps = (int)std::min<int64_t>(h->opt_warps_per_cta, warps);
@@ -445,7 +487,7 @@ static int walk4f_en_for(int ef, double s) {
 }
 
 // Can this filtered / deletion-aware search run on the two-list kernel?  (ep, en) = entries per lane of P and N.
-static bool walk4f_geometry(const annb_index *h, int ef, double selectivity, int *ep_out, int *en_out) {
+bool walk4f_geometry(const annb_index *h, int ef, double selectivity, int *ep_out, int *en_out) {
   if (h->opt_flagged_kernel == 1 || h->opt_flagged_epl > 0) return false;  // A/B and test switches: hnsw_walk_flagged
   if (!walk4_applicable(h) || h->gd.n >= (1ll << 30)) return false;
   if (ef > 128) return false;  // P wider than 4 entries per lane: the shared-memory merge of hnsw_walk_flagged
@@ -473,6 +515,33 @@ int launch_walk4f(annb_index *h, const SearchParams &p) {
     case 8: return launch_walk4f_m<8>(h, p, ep, en);
     case 16: return launch_walk4f_m<16>(h, p, ep, en);
     case 32: return launch_walk4f_m<32>(h, p, ep, en);
+  }
+  return 1;
+}
+
+// The filtered multi-cell walk (hnsw_walk4f<8, EP, EN, false, true>): p.ef = the caller's ef, p.cell_limit = the row
+// length of the scratch (>= every k_c), (ep, en) = the lists' entries per lane as walk4f_geometry gives them, chosen by
+// the caller to cover every walked cell; h = the handle whose stream and scratch the launch uses.  Only the fused table
+// build and M = 8 are instantiated.
+int launch_walk4f_cells(annb_index *h, const SearchParams &p, int ep, int en) {
+  if (p.B == 0) return ANNB_OK;
+  if (!p.queries || h->M != 8 || !p.cell_filter) return 1;
+  if (ep == 2) {
+    switch (en) {
+      case 2: return launch_walk4f_t<8, 2, 2, true>(h, p);
+      case 3: return launch_walk4f_t<8, 2, 3, true>(h, p);
+      case 4: return launch_walk4f_t<8, 2, 4, true>(h, p);
+      case 5: return launch_walk4f_t<8, 2, 5, true>(h, p);
+      case 6: return launch_walk4f_t<8, 2, 6, true>(h, p);
+      case 8: return launch_walk4f_t<8, 2, 8, true>(h, p);
+    }
+    return 1;
+  }
+  if (ep != 4) return 1;
+  switch (en) {
+    case 4: return launch_walk4f_t<8, 4, 4, true>(h, p);
+    case 6: return launch_walk4f_t<8, 4, 6, true>(h, p);
+    case 8: return launch_walk4f_t<8, 4, 8, true>(h, p);
   }
   return 1;
 }

@@ -375,6 +375,17 @@ class Engine:
     def filter_release(self, filter_id):
         L.check(self._lib.annb_filter_release(self._h, int(filter_id)))
 
+    def filter_prepare_labels(self, labels):
+        """A prepared filter from a label list (numpy, or a torch CUDA tensor) -> (filter id, count).  count = the
+        number of labels given, as a label-list filter counts them."""
+        if isinstance(labels, np.ndarray) or not hasattr(labels, 'data_ptr'):
+            labels = np.ascontiguousarray(np.asarray(labels).reshape(-1), dtype=np.uint64)
+        n = labels.shape[0]
+        lp, ls, _k = L.as_ptr(labels)
+        fid, cnt = C.c_int(), C.c_int64()
+        L.check(self._lib.annb_filter_prepare_labels(self._h, lp if n else None, n, ls, C.byref(fid), C.byref(cnt)))
+        return fid.value, cnt.value
+
     def search_prepared(self, queries, filter_id, k=10, ef=50, normalize=0, out_labels=None, out_dists=None):
         q = self._as_f32(queries)
         B = q.shape[0]
@@ -506,9 +517,12 @@ class CellSet:
         except Exception:
             pass
 
-    def search(self, queries, limit=10, ef=50, normalize=0, order=None, n_probe=None, generic=False, with_parts=False):
+    def search(self, queries, limit=10, ef=50, normalize=0, order=None, n_probe=None, generic=False, with_parts=False,
+               filter_ids=None):
         """-> (labels uint64 (B, limit), dists fp32 (B, limit), cells int32 (B, limit)) [+ (part labels, part dists,
-        part counters) (B, n_cells, limit / 3)].  `order` = (B, n_probe) cells per query, or None for the centroids'."""
+        part counters) (B, n_cells, limit / 3)].  `order` = (B, n_probe) cells per query, or None for the centroids'.
+        `filter_ids` = one prepared filter id per cell (of that cell's Engine; 0 = the cell admits nothing), or None
+        for no filter (annb_cellset_search_prepared / annb_cellset_search)."""
         q = Engine._as_f32(queries)
         B = q.shape[0]
         if order is not None:
@@ -527,11 +541,25 @@ class CellSet:
         qp, qs, _k = L.as_ptr(q)
         if order is not None and qs == L.DEVICE:
             raise ValueError('pass the probe order with host queries')
-        L.check(self._lib.annb_cellset_search(
-            self._h, qp, qs, B, int(normalize), order.ctypes.data if order is not None else None, n_probe, int(limit),
-            int(ef), L.CELLS_GENERIC if generic else 0, labels.ctypes.data, dists.ctypes.data, cells.ctypes.data, L.HOST,
-            *([p.ctypes.data for p in parts] if parts else [None, None, None])))
+        head = (self._h, qp, qs, B, int(normalize), order.ctypes.data if order is not None else None, n_probe, int(limit),
+                int(ef), L.CELLS_GENERIC if generic else 0)
+        tail = (labels.ctypes.data, dists.ctypes.data, cells.ctypes.data, L.HOST,
+                *([p.ctypes.data for p in parts] if parts else [None, None, None]))
+        if filter_ids is None:
+            L.check(self._lib.annb_cellset_search(*head, *tail))
+        else:
+            fids = np.ascontiguousarray(filter_ids, dtype=np.int32)
+            if fids.shape != (self.n_cells,):
+                raise ValueError(f'{fids.shape} filter ids for {self.n_cells} cells')
+            L.check(self._lib.annb_cellset_search_prepared(*head, fids.ctypes.data, *tail))
         return (labels, dists, cells) + ((parts,) if with_parts else ())
+
+    def last_filtered(self):
+        """What the last filtered search did besides the fused launch: (query, cell) pairs re-run on the bitmap walk,
+        and cells served by their own filtered launch."""
+        a, b = C.c_int64(), C.c_int()
+        L.check(self._lib.annb_cellset_last_filtered(self._h, C.byref(a), C.byref(b)))
+        return dict(rerun_pairs=a.value, handle_cells=b.value)
 
     def merge(self, labels, dists, counts, order, limit):
         """The merge alone over a by-cell scratch (host): labels / dists (B, n_cells, limit), counts (B, n_cells),

@@ -303,6 +303,12 @@ ANNB_API int annb_filter_prepare(annb_index_t *h, const annb_filter_op_t *progra
  * and sets *n_out = count. */
 ANNB_API int annb_filter_labels(annb_index_t *h, int filter_id, uint64_t *labels_out, int64_t cap, int64_t *n_out);
 ANNB_API int annb_filter_release(annb_index_t *h, int filter_id);
+/* A prepared filter from a label list (labels, n entries, host or device `space`): the bitmap a search with that list
+ * as filter_labels would walk, made once.  Its count is n, as a label list counts (repeats and labels not in the graph
+ * included), so annb_search_prepared with it returns what annb_search with the list returns.  It goes stale and is
+ * released like a program-prepared filter. */
+ANNB_API int annb_filter_prepare_labels(annb_index_t *h, const uint64_t *labels, int64_t n, int space, int *filter_id,
+                               int64_t *count);
 /* annb_search and annb_search_submit_filtered with a prepared filter in place of the label list: the bitmap is the
  * prepared one and the filter's size is its admitted count; everything else (kernel choice, list sizing, re-runs of
  * overflowing queries, ANNB_EFEWRESULTS) is the filtered route of those calls. */
@@ -394,6 +400,24 @@ ANNB_API int annb_cellset_search(annb_cellset_t *cs, const float *queries, int i
                         const int32_t *order, int n_probe, int limit, int ef, int flags, uint64_t *labels_out,
                         float *dists_out, int32_t *cells_out, int out_space, uint64_t *part_labels, float *part_dists,
                         int64_t *part_stats);
+/* annb_cellset_search with a filter per cell: filter_ids[c] (host, n_cells entries) = a prepared filter of cell c's
+ * handle (annb_filter_prepare*, live and not stale: ANNB_EINVAL / ANNB_ESTATE as annb_search_prepared), 0 = the cell
+ * admits nothing.  Cell c is searched with k_c = min(limit, its filter's count, its live rows) (skipped when 0) and
+ * ef_c = max(ef, k_c): what annb_search_prepared returns for the cell alone.  Where every cell has M = 8 / 256 u8
+ * codes and hnsw_walk4f's geometry for max(ef, limit), one launch builds each query's ADC table once and walks all its
+ * probed cells with their bitmaps (hnsw_walk4f's multi-cell form, its traversed-only list sized for the most selective
+ * cell it walks); a cell too selective for hnsw_walk4f gets the filtered launch annb_search_prepared would run for it,
+ * and (query, cell) pairs that outgrew the list are re-run on the bitmap walk of their cell, all on the device.  A
+ * probed walk with fewer than k_c results gives ANNB_EFEWRESULTS.  Other geometries, ef > 128 or ANNB_CELLS_GENERIC
+ * take one annb_search_prepared per probed cell (whose ANNB_EFEWRESULTS is returned).  Merge, outputs and parts as
+ * annb_cellset_search. */
+ANNB_API int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int in_space, int64_t B, int normalize,
+                                 const int32_t *order, int n_probe, int limit, int ef, int flags, const int *filter_ids,
+                                 uint64_t *labels_out, float *dists_out, int32_t *cells_out, int out_space,
+                                 uint64_t *part_labels, float *part_dists, int64_t *part_stats);
+/* What the last annb_cellset_search_prepared did besides the fused launch: (query, cell) pairs re-run on the bitmap
+ * walk, and cells served by their own filtered launch. */
+ANNB_API int annb_cellset_last_filtered(annb_cellset_t *cs, int64_t *rerun_pairs, int *handle_cells);
 ANNB_API int annb_cellset_merge(annb_cellset_t *cs, const uint64_t *labels, const float *dists, const int32_t *counts,
                        const int32_t *order, int in_space, int64_t B, int n_probe, int limit, uint64_t *labels_out,
                        float *dists_out, int32_t *cells_out, int out_space);
