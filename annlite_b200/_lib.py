@@ -87,6 +87,8 @@ PROTOTYPES = {
     'annb_cellset_search': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp]),
     'annb_cellset_search_prepared': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _int,
                                             _vp, _vp, _vp]),
+    'annb_cellset_search_multi': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _int,
+                                         _vp, _vp, _vp]),
     'annb_cellset_last_filtered': (_int, [_vp, C.POINTER(_i64), C.POINTER(_int)]),
     'annb_cellset_merge': (_int, [_vp, _vp, _vp, _vp, _vp, _int, _i64, _int, _int, _vp, _vp, _vp, _int]),
     'annb_cellset_probe': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int]),

@@ -6,9 +6,9 @@ Differences from the reference, besides the docarray / SQLite / RocksDB stores i
   map stands in for the MetaTable.  Results carry those labels, not doc ids looked up per cell offset.
 * a batch of queries runs as one GPU search (annb_cellset_search): without a filter or deletions, one launch builds
   each query's ADC table once and walks all its probed cells.  A dict filter or an id array is prepared on each probed
-  cell and searched the same way with each cell's bitmap (annb_cellset_search_prepared), deletions included.  Per-query
-  filter lists, cells with `bruteforce_filter_below` set and unfiltered searches after deletions search the cells one
-  by one.
+  cell and searched the same way with each cell's bitmap (annb_cellset_search_prepared), deletions included; a list
+  of per-query filter dicts too, each query with its own bitmap in each cell (annb_cellset_search_multi).  Cells with
+  `bruteforce_filter_below` set and unfiltered searches after deletions search the cells one by one.
 * equal distances in the merge keep concatenation order (the reference's argsort leaves them unspecified); a query
   with fewer than `limit` results is padded with +inf / UINT64_MAX / cell -1.
 * with a VQCodec attached, cells are probed in the order of annlite.math.cdist over the centroids.  The reference's
@@ -181,8 +181,12 @@ class CellContainer:
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
                                        generic=generic)
             return dist, lab, cid
-        if (not generic and not is_per_query_filter(filter)
-                and all(v.bruteforce_filter_below is None for v in self._vec_indexes)):
+        per_query = is_per_query_filter(filter)
+        if per_query and len(filter) != B:
+            raise ValueError(f'{len(filter)} filters for {B} queries')
+        if not generic and all(v.bruteforce_filter_below is None for v in self._vec_indexes):
+            if per_query:
+                return self._search_cells_multi(x, cells, filter, limit)
             return self._search_cells_prepared(x, cells, filter, limit)
         # filtered, per-cell route: one filtered search per probed cell (HnswIndex.search_batch shrinks the limit to
         # what the filter admits there, hnsw/index.py:151-154), then the same merge on the GPU
@@ -251,6 +255,28 @@ class CellContainer:
                 fids[c] = prepared[-1].id
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
                                        filter_ids=fids)
+        finally:
+            for p in prepared:
+                p.release()
+        return dist, lab, cid
+
+    def _search_cells_multi(self, x, cells, filters, limit):
+        """One filter dict per query over the probed cells in one GPU search (annb_cellset_search_multi): the list is
+        prepared on each probed cell with rows (HnswIndex.prepare_filters), whose ids form that cell's column of the
+        (B, n_cells) table; every pair's k is what the per-cell route's search_batch uses: min(limit, live rows,
+        admitted count).  Cells not probed or empty keep a column of 0s (their k is 0 through the live count)."""
+        cs = self._cells()
+        v0 = self._vec_indexes[0]
+        qids = np.zeros((x.shape[0], self.n_cells), dtype=np.int32)
+        prepared = []
+        try:
+            for c in np.unique(cells).tolist():
+                if self._live[c] == 0:
+                    continue
+                prepared.append(self._vec_indexes[c].prepare_filters(filters))
+                qids[:, c] = prepared[-1].ids
+            lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
+                                       query_filter_ids=qids)
         finally:
             for p in prepared:
                 p.release()

@@ -155,6 +155,10 @@ struct SearchParams {
   // filtered multi-cell walk (hnsw_walk4f<8, EP, EN, false, true>, annb_cellset_search_prepared): the device array of
   // the cells' prepared bitmaps by internal id, one per cell
   const uint32_t *const *cell_filter;
+  // per-query filtered multi-cell walk (hnsw_walk4f<8, EP, EN, true, true>, annb_cellset_search_multi): each query's
+  // slot (B); cell_k and cell_filter are then (slots, n_cells) tables, and a cell_filter entry carries its reading in
+  // its low bits (bit 0 = "not deleted", bit 1 = size guard), nullptr here = the forms above
+  const int32_t *query_slot;
 };
 
 // ------------------------------------------------------------------------------------------

@@ -10,6 +10,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <map>
 #include <vector>
 
 #include "annb_internal.h"
@@ -20,19 +21,20 @@ struct annb_cellset {
   annb_index *h0 = nullptr;         // its stream and scratch serve the cell set's launches
   float *d_centroids = nullptr;     // (n_cells, dim) or nullptr (then every search needs an explicit order)
   GraphDev *d_graphs = nullptr;     // (n_cells) descriptors, re-read before every fused search
-  void *buf[16] = {nullptr};
-  size_t cap[16] = {0};
+  void *buf[24] = {nullptr};
+  size_t cap[24] = {0};
   float probe_ms = 0, walk_ms = 0, merge_ms = 0;
   cudaEvent_t ev[8] = {nullptr};    // [0,1] probe, [2,3] walk, [4,5] merge, [6,7] hand-over to a cell's stream and back
   int last_route = 0;
-  int64_t last_rerun_pairs = 0;     // annb_cellset_search_prepared: (query, cell) pairs re-run on the bitmap walk
+  int64_t last_rerun_pairs = 0;     // annb_cellset_search_prepared / _multi: (query, cell) pairs re-run on the bitmap walk
   int last_handle_cells = 0;        // ... and cells served by their own filtered launch instead of the fused walk
 };
 
 namespace {
 
 enum { C_QUERIES = 0, C_ORDER, C_K, C_LABELS, C_DISTS, C_FOUND, C_STATS, C_OUT, C_BITS, C_TABLES, C_TMP_L, C_TMP_D, C_TMP_F,
-       C_TMP_S, C_QMAP };
+       C_TMP_S, C_QMAP, C_SLOT, C_SLOT_K, C_SLOT_BITS, C_GTABLES, C_QF };
+static_assert(C_QF < 24, "annb_cellset::buf is too small");
 
 int cs_buf(annb_cellset *cs, int slot, size_t bytes, void **out) {
   if (bytes == 0) bytes = 16;
@@ -297,33 +299,34 @@ int host_order(annb_cellset *cs, const int32_t *order, int in_space, const int32
 }
 
 // rows of one cell's (B, k) search outputs -> that cell's rows (q * n_cells + c) of the by-cell scratch: every row, or
-// (idx) the rows a re-run wrote, idx[i] = query row
+// (idx) the rows a re-run wrote, idx[i] = query row; `dense` = the outputs hold only those rows, row i for query idx[i]
 __global__ void cell_scatter_kernel(const uint64_t *__restrict__ il, const float *__restrict__ id, const int32_t *__restrict__ ifound,
                                     const int64_t *__restrict__ istats, const uint32_t *__restrict__ idx, int64_t n, int k,
-                                    int n_cells, int c, int stride, uint64_t *__restrict__ sl, float *__restrict__ sd,
+                                    int n_cells, int c, int stride, int dense, uint64_t *__restrict__ sl, float *__restrict__ sd,
                                     int32_t *__restrict__ sfound, int64_t *__restrict__ sstats) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t i = t / k;
   if (i >= n) return;
   const int j = (int)(t - i * k);
   const int64_t q = idx ? (int64_t)idx[i] : i;
+  const int64_t r = dense ? i : q;  // input row
   const int64_t o = q * n_cells + c;
-  sl[o * stride + j] = il[q * k + j];
-  sd[o * stride + j] = id[q * k + j];
+  sl[o * stride + j] = il[r * k + j];
+  sd[o * stride + j] = id[r * k + j];
   if (j == 0) {
-    sfound[o] = ifound[q];
+    sfound[o] = ifound[r];
     if (sstats)
-      for (int s = 0; s < 3; s++) sstats[o * 3 + s] = istats[q * 3 + s];
+      for (int s = 0; s < 3; s++) sstats[o * 3 + s] = istats[r * 3 + s];
   }
 }
 
 int launch_cell_scatter(cudaStream_t st, const uint64_t *il, const float *id, const int32_t *ifound, const int64_t *istats,
                         const uint32_t *idx, int64_t n, int k, int n_cells, int c, int stride, uint64_t *sl, float *sd,
-                        int32_t *sfound, int64_t *sstats) {
+                        int32_t *sfound, int64_t *sstats, bool dense = false) {
   if (n == 0) return ANNB_OK;
   const int64_t total = n * k;
-  cell_scatter_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(il, id, ifound, istats, idx, n, k, n_cells, c, stride, sl, sd,
-                                                                        sfound, sstats);
+  cell_scatter_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(il, id, ifound, istats, idx, n, k, n_cells, c, stride,
+                                                                        dense ? 1 : 0, sl, sd, sfound, sstats);
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;
 }
@@ -730,6 +733,275 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
         if (walked[q * C + c] && kc[c] > 0 && hfound[q * C + c] < kc[c])
           ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   }
+  return merge_and_finish(cs, b.sd, b.sl, b.sfound, b.sstats, b.dorder, !order, B, n_probe, limit, labels_out, dists_out, cells_out,
+                          out_space, part_labels, part_dists, part_stats);
+}
+
+// The search over a cell set with a filter per query: query q admits in cell c the rows of cell c's prepared filter
+// query_filter[q * n_cells + c] (0 = no filter there: the live rows).  Each (query, cell) pair is what
+// annb_search_multi does for that query on that cell alone, with k = min(limit, admitted rows, live rows) (no filter:
+// min(limit, live rows)) and ef = max(ef, k).  Identical rows of the id table share a slot, so the walk's per-pair
+// tables are (slots, n_cells).  Fused route (every cell M = 8, 256 u8 codes, hnsw_walk4f geometry for max(ef, limit)):
+// one launch of hnsw_walk4f's per-query multi-cell form over every probed pair whose selectivity hnsw_walk4f covers at
+// its ef, N sized for the most selective of them; the other pairs get their cell's own launch over their rows (the
+// kernel annb_search_multi picks for them, over K1 tables, one launch per distinct k and kind of filter); pairs any walk
+// flagged are re-run on their cell's bitmap walk with their own bitmap.  Other geometries, ef > 128 and
+// ANNB_CELLS_GENERIC send every pair to its cell's own launch.  Everything runs on the device, then the merge.
+int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_space, int64_t B, int normalize,
+                              const int32_t *order, int n_probe, int limit, int ef, int flags, const int *query_filter,
+                              uint64_t *labels_out, float *dists_out, int32_t *cells_out, int out_space,
+                              uint64_t *part_labels, float *part_dists, int64_t *part_stats) {
+  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  const int C = cs->n_cells;
+  if (B < 0 || limit <= 0 || ef <= 0 || !labels_out || !dists_out || !cells_out || (B > 0 && !queries) || !query_filter)
+    ANNB_FAIL(ANNB_EINVAL, "bad B / limit / ef / outputs / filter ids");
+  if (n_probe < 1 || n_probe > C) ANNB_FAIL(ANNB_EINVAL, "n_probe=%d outside 1..n_cells=%d", n_probe, C);
+  if (!order && !cs->d_centroids) ANNB_FAIL(ANNB_ESTATE, "no centroids: pass the probe order");
+  const int ef_max = std::max(ef, limit);
+  if (ef_max > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, limit)=%d exceeds ANNB_MAX_EF=%d", ef_max, ANNB_MAX_EF);
+  if ((double)B * C >= 2147483647.0) ANNB_FAIL(ANNB_ELIMIT, "B x n_cells=%lld exceeds 2^31-1", (long long)B * C);
+  if (order && in_space != ANNB_DEVICE) ANNB_TRY_RC(check_order(order, B, n_probe, C));
+  annb_index *h0 = cs->h0;
+  ANNB_CUDA(cudaSetDevice(h0->device));
+  // slots: the distinct rows of the id table, each represented by its first query
+  std::vector<int32_t> slot((size_t)B);
+  std::vector<int64_t> srep;
+  {
+    std::unordered_map<std::string, int32_t> seen;
+    for (int64_t q = 0; q < B; q++) {
+      auto it = seen.emplace(std::string((const char *)(query_filter + q * C), (size_t)C * sizeof(int)), (int32_t)srep.size());
+      if (it.second) srep.push_back(q);
+      slot[(size_t)q] = it.first->second;
+    }
+  }
+  const int64_t S = (int64_t)srep.size();
+  auto row_id = [&](int64_t s, int c) { return query_filter[srep[(size_t)s] * C + c]; };
+  // every cell's device graph up to date, its filters resolved; per (slot, cell): k, bitmap, selectivity
+  std::vector<GraphDev> gd(C);
+  std::vector<int64_t> ndel(C);
+  std::vector<int32_t> sk((size_t)(S * C), 0);
+  std::vector<const uint32_t *> sbits((size_t)(S * C), nullptr);  // nullptr = no filter in this cell
+  std::vector<float> ssel((size_t)(S * C), 1.f);
+  bool fused = !(flags & ANNB_CELLS_GENERIC);
+  for (int c = 0; c < C; c++) {
+    annb_index *h = cs->cells[c];
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "cell %d: index not initialised", c);
+    ANNB_TRY_RC(sync_device_graph(h));
+    ANNB_CUDA(cudaStreamSynchronize(h->stream));
+    ANNB_CUDA(cudaStreamSynchronize(h->stream2));
+    gd[c] = h->gd;
+    ndel[c] = h->g.num_deleted;
+    const int64_t live = std::max<int64_t>(h->g.count.load() - h->g.num_deleted, 0);
+    const double nn = (double)std::max<int64_t>(1, h->gd.n);
+    std::unordered_map<int, const PreparedFilter *> pf;
+    for (int64_t s = 0; s < S; s++) {
+      const int id = row_id(s, c);
+      const size_t i = (size_t)(s * C + c);
+      if (id == 0) {  // annb_search_multi's unfiltered rows: the live rows (k = min(limit, live), container.py:119)
+        sk[i] = (int32_t)std::min<int64_t>(limit, live);
+        ssel[i] = (float)(1.0 - (double)h->g.num_deleted / nn);
+        continue;
+      }
+      auto it = pf.find(id);
+      if (it == pf.end()) {
+        PreparedFilter *f;
+        const int rc = find_prepared_filter(h, id, &f);
+        if (rc) {
+          const std::string msg = annb_last_error();
+          ANNB_FAIL(rc, "cell %d: %s", c, msg.c_str());
+        }
+        if ((int)pf.size() >= ANNB_FILTER_MAX_PER_CALL)
+          ANNB_FAIL(ANNB_ELIMIT, "cell %d: more than %d distinct filters in one call", c, ANNB_FILTER_MAX_PER_CALL);
+        it = pf.emplace(id, f).first;
+      }
+      const PreparedFilter *f = it->second;
+      sk[i] = (int32_t)std::min<int64_t>({(int64_t)limit, f->count, live});
+      sbits[i] = f->bits;
+      ssel[i] = (float)std::min<double>(1.0, (double)f->count / nn);
+    }
+    int ep, en;
+    fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
+  }
+  cs->last_route = fused ? 0 : 1;
+  cs->last_rerun_pairs = 0;
+  cs->last_handle_cells = 0;
+  if (B == 0) return ANNB_OK;
+  cudaStream_t st = h0->stream;
+  Staged b;
+  ANNB_TRY_RC(stage_batch(cs, queries, in_space, B, order, n_probe, limit, part_stats != nullptr, b));
+  for (int r = 0; r < normalize; r++) ANNB_TRY_RC(launch_l2_normalize(h0, b.dq, B, cs->dim));
+  std::vector<int32_t> otmp;
+  const int32_t *ho;
+  ANNB_TRY_RC(host_order(cs, order, in_space, b.dorder, B, n_probe, otmp, &ho));
+  // the pairs walked: probed, with k > 0 (and which slots probe which cells)
+  std::vector<char> walked((size_t)(B * C), 0), sprobed((size_t)(S * C), 0);
+  for (int64_t q = 0; q < B; q++)
+    for (int i = 0; i < n_probe; i++) {
+      const int c = ho[q * n_probe + i];
+      const size_t sc = (size_t)slot[(size_t)q] * C + c;
+      sprobed[sc] = 1;
+      walked[(size_t)(q * C + c)] = sk[sc] > 0;
+    }
+  // fused route: the pairs hnsw_walk4f serves, and N's size (the largest any of them needs alone)
+  std::vector<char> own((size_t)(S * C), 0);  // 1 = the pair goes to its cell's own launch
+  int ep = ef_max <= 64 ? 2 : 4, en = 0;
+  for (int64_t s = 0; s < S; s++)
+    for (int c = 0; c < C; c++) {
+      const size_t i = (size_t)(s * C + c);
+      if (!sprobed[i] || sk[i] == 0) continue;
+      int ep_c, en_c;
+      if (fused && walk4f_geometry(cs->cells[c], std::max(ef, sk[i]), (double)ssel[i], &ep_c, &en_c)) en = std::max(en, en_c);
+      else own[i] = 1;
+    }
+  if (ep == 4 && en > 0) en = en <= 4 ? 4 : (en <= 6 ? 6 : 8);
+  cudaEventRecord(cs->ev[2], st);
+  if (en > 0) {
+    // the walk's tables: k per (slot, cell) (0 = skip, own-launch pairs included) and the admission word: the filter's
+    // bitmap, or (no filter) the cell's deletions read as "not deleted", with the size guard when there are any
+    std::vector<int32_t> kwalk(sk);
+    std::vector<uintptr_t> word((size_t)(S * C));
+    for (size_t i = 0; i < word.size(); i++) {
+      const int c = (int)(i % C);
+      if (own[i]) kwalk[i] = 0;
+      const uint32_t *bits = sbits[i] ? sbits[i] : gd[c].deleted;  // (sync_device_graph always uploads the deletions)
+      if (kwalk[i] > 0 && (!bits || (reinterpret_cast<uintptr_t>(bits) & 3u)))
+        ANNB_FAIL(ANNB_ESTATE, "internal: cell %d has no 4-byte aligned admission bitmap", c);
+      word[i] = reinterpret_cast<uintptr_t>(bits) | (sbits[i] ? 0u : 1u | (ndel[c] > 0 ? 2u : 0u));
+    }
+    int32_t *dslot, *dk;
+    uintptr_t *dword;
+    ANNB_TRY_RC(cs_buf(cs, C_SLOT, (size_t)B * 4, (void **)&dslot));
+    ANNB_TRY_RC(cs_buf(cs, C_SLOT_K, kwalk.size() * 4, (void **)&dk));
+    ANNB_TRY_RC(cs_buf(cs, C_SLOT_BITS, word.size() * sizeof(uintptr_t), (void **)&dword));
+    ANNB_CUDA(cudaMemcpyAsync(cs->d_graphs, gd.data(), sizeof(GraphDev) * C, cudaMemcpyHostToDevice, st));
+    ANNB_CUDA(cudaMemcpyAsync(dslot, slot.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st));
+    ANNB_CUDA(cudaMemcpyAsync(dk, kwalk.data(), kwalk.size() * 4, cudaMemcpyHostToDevice, st));
+    ANNB_CUDA(cudaMemcpyAsync(dword, word.data(), word.size() * sizeof(uintptr_t), cudaMemcpyHostToDevice, st));
+    SearchParams p;
+    cells_params(cs, b, B, n_probe, limit, ef, dk, p);
+    p.cell_filter = reinterpret_cast<const uint32_t *const *>(dword);
+    p.query_slot = dslot;
+    std::lock_guard<std::mutex> lk(h0->mu);
+    const int rc = launch_walk4f_cells(h0, p, ep, en);
+    if (rc == 1) ANNB_FAIL(ANNB_ESTATE, "the per-query filtered multi-cell walk does not apply to these cells");
+    if (rc) return rc;
+  }
+  // the K1 tables of the whole batch, for the own launches and the re-runs (built once)
+  const int TS = h0->M * h0->Ks;
+  float *tables = nullptr;
+  auto need_tables = [&]() -> int {
+    if (tables) return ANNB_OK;
+    ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * TS * sizeof(float), (void **)&tables));
+    std::lock_guard<std::mutex> lk(h0->mu);
+    return launch_adc_table(h0, b.dq, B, tables);
+  };
+  // one launch of cell c over query rows `rows` (their tables gathered) with k, on its own handle's stream (after
+  // everything queued on the cell set's, which waits for it in turn); `qf` = each row's bitmap (nullptr = no filter),
+  // or empty for a launch without per-query filters; its outputs scattered into the rows' pairs of the scratch
+  auto rows_launch = [&](int c, int mode, int k, float sel, const std::vector<uint32_t> &rows,
+                         const std::vector<const uint32_t *> &qf) -> int {
+    annb_index *h = cs->cells[c];
+    const int64_t n = (int64_t)rows.size();
+    ANNB_TRY_RC(need_tables());
+    uint64_t *tl;
+    float *td, *gt;
+    int32_t *tf;
+    int64_t *ts = nullptr;
+    uint32_t *dmap;
+    const uint32_t **dqf = nullptr;
+    ANNB_TRY_RC(cs_buf(cs, C_TMP_L, (size_t)n * k * 8, (void **)&tl));
+    ANNB_TRY_RC(cs_buf(cs, C_TMP_D, (size_t)n * k * 4, (void **)&td));
+    ANNB_TRY_RC(cs_buf(cs, C_TMP_F, (size_t)n * 4, (void **)&tf));
+    if (b.sstats) ANNB_TRY_RC(cs_buf(cs, C_TMP_S, (size_t)n * 24, (void **)&ts));
+    ANNB_TRY_RC(cs_buf(cs, C_GTABLES, (size_t)n * TS * sizeof(float), (void **)&gt));
+    ANNB_TRY_RC(cs_buf(cs, C_QMAP, (size_t)n * 4, (void **)&dmap));
+    ANNB_CUDA(cudaMemcpyAsync(dmap, rows.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    if (!qf.empty()) {
+      ANNB_TRY_RC(cs_buf(cs, C_QF, (size_t)n * sizeof(void *), (void **)&dqf));
+      ANNB_CUDA(cudaMemcpyAsync(dqf, qf.data(), (size_t)n * sizeof(void *), cudaMemcpyHostToDevice, st));
+    }
+    SearchParams p;
+    memset(&p, 0, sizeof(p));
+    p.tables = gt;
+    p.B = n;
+    p.k = k;
+    p.ef = std::max(ef, k);
+    p.query_filter = dqf;
+    p.selectivity = sel;
+    p.out_labels = tl;
+    p.out_dists = td;
+    p.out_found = tf;
+    p.out_stats = ts;
+    std::lock_guard<std::mutex> lk(h->mu);
+    ANNB_CUDA(cudaEventRecord(cs->ev[6], st));
+    ANNB_CUDA(cudaStreamWaitEvent(h->stream, cs->ev[6], 0));
+    ANNB_TRY_RC(launch_rows_copy(h, tables, gt, dmap, n, TS, false));
+    ANNB_TRY_RC(launch_search(h, p, mode));
+    ANNB_TRY_RC(launch_cell_scatter(h->stream, tl, td, tf, ts, dmap, n, k, C, c, limit, b.sl, b.sd, b.sfound, b.sstats, true));
+    ANNB_CUDA(cudaEventRecord(cs->ev[7], h->stream));
+    ANNB_CUDA(cudaStreamWaitEvent(st, cs->ev[7], 0));
+    return ANNB_OK;
+  };
+  // own launches, cell by cell: one per (k, kind) -- kind 0 = no filter (annb_search_multi's plain or deletion-aware
+  // group), 1 = filters hnsw_walk4f takes at that ef, 2 = the others -- as annb_search_multi groups the same rows
+  for (int c = 0; c < C; c++) {
+    annb_index *h = cs->cells[c];
+    struct Group {
+      std::vector<uint32_t> rows;
+      std::vector<const uint32_t *> qf;
+      double s = 1.0;
+    };
+    std::map<std::pair<int, int>, Group> groups;
+    for (int64_t q = 0; q < B; q++) {
+      const size_t i = (size_t)slot[(size_t)q] * C + c;
+      if (!walked[(size_t)(q * C + c)] || !own[i]) continue;
+      const int k = sk[i];
+      const int kind = !sbits[i] ? 0 : ((h->opt_force_general != 2 && walk4f_applicable(h, std::max(ef, k), ssel[i])) ? 1 : 2);
+      Group &g = groups[{k, kind}];
+      g.rows.push_back((uint32_t)q);
+      if (kind) g.qf.push_back(sbits[i]);
+      g.s = std::min(g.s, (double)ssel[i]);
+    }
+    for (auto &kv : groups) {
+      const int k = kv.first.first, kind = kv.first.second;
+      int mode = h->opt_force_general == 2 ? 2 : 1;
+      if (kind == 0 && ndel[c] == 0 && !h->opt_force_general) mode = 0;
+      ANNB_TRY_RC(rows_launch(c, mode, k, (float)kv.second.s, kv.second.rows, kv.second.qf));
+    }
+    if (!groups.empty()) cs->last_handle_cells++;
+  }
+  // pairs a walk flagged (found = -1): re-run on the bitmap walk of their cell with their own bitmap, one launch per
+  // (cell, k)
+  std::vector<int32_t> hfound((size_t)(B * C));
+  ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
+  ANNB_CUDA(cudaStreamSynchronize(st));
+  int64_t reruns = 0;
+  for (int c = 0; c < C; c++) {
+    std::map<int, std::pair<std::vector<uint32_t>, std::vector<const uint32_t *>>> over;
+    for (int64_t q = 0; q < B; q++) {
+      if (!walked[(size_t)(q * C + c)] || hfound[(size_t)(q * C + c)] >= 0) continue;
+      const size_t i = (size_t)slot[(size_t)q] * C + c;
+      auto &o = over[sk[i]];
+      o.first.push_back((uint32_t)q);
+      o.second.push_back(sbits[i]);
+    }
+    for (auto &kv : over) {
+      ANNB_TRY_RC(rows_launch(c, 2, kv.first, 1.f, kv.second.first, kv.second.second));
+      reruns += (int64_t)kv.second.first.size();
+    }
+  }
+  cudaEventRecord(cs->ev[3], st);
+  cs->last_rerun_pairs = reruns;
+  if (reruns) {
+    ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
+    ANNB_CUDA(cudaStreamSynchronize(st));
+  }
+  // a walk with fewer than k results: the cell's own annb_search_multi would fail with ANNB_EFEWRESULTS
+  for (int64_t q = 0; q < B; q++)
+    for (int c = 0; c < C; c++)
+      if (walked[(size_t)(q * C + c)] && hfound[(size_t)(q * C + c)] < sk[(size_t)slot[(size_t)q] * C + c])
+        ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   return merge_and_finish(cs, b.sd, b.sl, b.sfound, b.sstats, b.dorder, !order, B, n_probe, limit, labels_out, dists_out, cells_out,
                           out_space, part_labels, part_dists, part_stats);
 }

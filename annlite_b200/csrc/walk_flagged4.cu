@@ -76,6 +76,13 @@ constexpr int w4f_min_ctas(int M, int EP, int EN) {  // register cap = 64K / (ma
 // no size guard) with k_c = p.cell_k[c] (0 = skip the cell) and ef_c = max(ef, k_c).  Results, found and counters go to
 // row q * n_cells + c of the by-cell scratch; a (query, cell) walk that outgrows N writes found = -1 for that pair only
 // and the query goes on with its next cell.  `g_in` and `has_del` are unused then.
+//
+// PQF and CELLS: the per-query filtered multi-cell walk of annb_cellset_search_multi.  Query q belongs to slot
+// s = p.query_slot[q] (queries with the same filter in every cell share one); cell c is walked with the pair's
+// k = p.cell_k[s * n_cells + c] (0 = skip) and admission word p.cell_filter[s * n_cells + c], a bitmap pointer whose
+// low bits say how to read it: bit 0 = "not deleted" (flip, the query has no filter in this cell: the bitmap is the
+// cell's deletions), bit 1 = the size guard of :270 (the cell has deletions).  Without either bit it is a prepared
+// filter with filter semantics, as in the CELLS form.
 template <int M, int EP, int EN, bool PQF, bool CELLS>
 __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP, EN))
     hnsw_walk4f(const GraphDev g_in, const SearchParams p, const int has_del) {
@@ -137,7 +144,7 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
     const int64_t q = __reduce_max_sync(FULL_MASK, qi);
     if (q >= p.B) break;
     __syncwarp();
-    if constexpr (PQF) {
+    if constexpr (PQF && !CELLS) {
       const uint32_t *f = p.query_filter[q];
       use_filter = f != nullptr;
       bits = use_filter ? f : g_in.deleted;
@@ -161,11 +168,14 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       for (int i = lane; i < TS; i += 32) o[i] = T[i];
     }
 
+    int slot_row = 0;  // PQF && CELLS: first entry of the query's slot in the (slot, cell) tables
+    if constexpr (PQF && CELLS) slot_row = __ldg(p.query_slot + q) * p.n_cells;
     for (int ci = 0; ci < (CELLS ? p.n_probe : 1); ci++) {
     int64_t oq = q;  // output row
     if constexpr (CELLS) {
       const int c = __ldg(p.cell_order + q * p.n_probe + ci);
-      k = __ldg(p.cell_k + c);
+      if constexpr (PQF) k = __ldg(p.cell_k + slot_row + c);
+      else k = __ldg(p.cell_k + c);
       oq = q * p.n_cells + c;
       if (k == 0) {  // nothing admitted: the cell is skipped
         if (lane0) p.out_found[oq] = 0;
@@ -175,7 +185,14 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       ef = max(p.ef, k);  // hnswalg.h:1279
       wl = (ef - 1) / EP;
       ws = (ef - 1) % EP;
-      bits = p.cell_filter[c];
+      if constexpr (PQF) {
+        const uintptr_t w = reinterpret_cast<uintptr_t>(p.cell_filter[slot_row + c]);
+        bits = reinterpret_cast<const uint32_t *>(w & ~(uintptr_t)3);
+        flip = (uint32_t)(w & 1u);
+        size_guard = (w & 2u) != 0;
+      } else {
+        bits = p.cell_filter[c];
+      }
       has_slot0 = lane < gc.maxM0;
       uint64_t t = reinterpret_cast<uint64_t>(gc.rec0 + 4 * lane);
       asm volatile("" : "+l"(t));
@@ -423,7 +440,7 @@ int launch_walk4f_t(annb_index *h, const SearchParams &p_in) {
   SearchParams p = p_in;
   static_assert(w4f_fits(M, EP, EN, true) && w4f_fits(M, EP, EN, false), "walk4f geometry exceeds the SM's shared memory");
   void (*kern)(const GraphDev, const SearchParams, const int);
-  if constexpr (CELLS) kern = hnsw_walk4f<M, EP, EN, false, true>;
+  if constexpr (CELLS) kern = p.query_slot ? hnsw_walk4f<M, EP, EN, true, true> : hnsw_walk4f<M, EP, EN, false, true>;
   else kern = p.query_filter ? hnsw_walk4f<M, EP, EN, true, false> : hnsw_walk4f<M, EP, EN, false, false>;
   const bool fused = p.queries != nullptr;
   int warps = w4f_cta_warps(M, EP, EN, fused), ctas = w4f_ctas(M, EP, EN, fused);
@@ -522,7 +539,8 @@ int launch_walk4f(annb_index *h, const SearchParams &p) {
 // The filtered multi-cell walk (hnsw_walk4f<8, EP, EN, false, true>): p.ef = the caller's ef, p.cell_limit = the row
 // length of the scratch (>= every k_c), (ep, en) = the lists' entries per lane as walk4f_geometry gives them, chosen by
 // the caller to cover every walked cell; h = the handle whose stream and scratch the launch uses.  Only the fused table
-// build and M = 8 are instantiated.
+// build and M = 8 are instantiated.  With p.query_slot set, the per-query form (hnsw_walk4f<8, EP, EN, true, true>):
+// p.cell_k and p.cell_filter are then (slots, n_cells) tables.
 int launch_walk4f_cells(annb_index *h, const SearchParams &p, int ep, int en) {
   if (p.B == 0) return ANNB_OK;
   if (!p.queries || h->M != 8 || !p.cell_filter) return 1;

@@ -518,11 +518,13 @@ class CellSet:
             pass
 
     def search(self, queries, limit=10, ef=50, normalize=0, order=None, n_probe=None, generic=False, with_parts=False,
-               filter_ids=None):
+               filter_ids=None, query_filter_ids=None):
         """-> (labels uint64 (B, limit), dists fp32 (B, limit), cells int32 (B, limit)) [+ (part labels, part dists,
         part counters) (B, n_cells, limit / 3)].  `order` = (B, n_probe) cells per query, or None for the centroids'.
         `filter_ids` = one prepared filter id per cell (of that cell's Engine; 0 = the cell admits nothing), or None
-        for no filter (annb_cellset_search_prepared / annb_cellset_search)."""
+        for no filter (annb_cellset_search_prepared / annb_cellset_search).  `query_filter_ids` = (B, n_cells): a
+        prepared filter id of cell c's Engine for query q (0 = no filter for that query there), one filter per query
+        (annb_cellset_search_multi); exclusive with `filter_ids`."""
         q = Engine._as_f32(queries)
         B = q.shape[0]
         if order is not None:
@@ -545,7 +547,14 @@ class CellSet:
                 int(ef), L.CELLS_GENERIC if generic else 0)
         tail = (labels.ctypes.data, dists.ctypes.data, cells.ctypes.data, L.HOST,
                 *([p.ctypes.data for p in parts] if parts else [None, None, None]))
-        if filter_ids is None:
+        if filter_ids is not None and query_filter_ids is not None:
+            raise ValueError('pass filter_ids or query_filter_ids, not both')
+        if query_filter_ids is not None:
+            qids = np.ascontiguousarray(query_filter_ids, dtype=np.int32)
+            if qids.shape != (B, self.n_cells):
+                raise ValueError(f'query filter ids of shape {qids.shape} for {B} queries and {self.n_cells} cells')
+            L.check(self._lib.annb_cellset_search_multi(*head, qids.ctypes.data, *tail))
+        elif filter_ids is None:
             L.check(self._lib.annb_cellset_search(*head, *tail))
         else:
             fids = np.ascontiguousarray(filter_ids, dtype=np.int32)

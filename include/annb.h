@@ -415,8 +415,24 @@ ANNB_API int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queri
                                  const int32_t *order, int n_probe, int limit, int ef, int flags, const int *filter_ids,
                                  uint64_t *labels_out, float *dists_out, int32_t *cells_out, int out_space,
                                  uint64_t *part_labels, float *part_dists, int64_t *part_stats);
-/* What the last annb_cellset_search_prepared did besides the fused launch: (query, cell) pairs re-run on the bitmap
- * walk, and cells served by their own filtered launch. */
+/* annb_cellset_search with a filter per query: query_filter (host, (B, n_cells)) entry q * n_cells + c = a prepared
+ * filter of cell c's handle (annb_filter_prepare_many; live and not stale: ANNB_EINVAL / ANNB_ESTATE, the message
+ * names the cell), 0 = query q has no filter in cell c.  Each (query, cell) pair is what annb_search_multi returns for
+ * that query on that cell alone: k = min(limit, the filter's count, the cell's live rows), without a filter
+ * min(limit, live rows) (skipped when 0), ef = max(ef, k); deleted rows are left out.  Identical rows of the table
+ * share one slot.  Where every cell has M = 8 / 256 u8 codes and hnsw_walk4f's geometry for max(ef, limit), one launch
+ * builds each query's ADC table once and walks all its probed cells with the pair's bitmap (hnsw_walk4f's per-query
+ * multi-cell form, its traversed-only list sized for the most selective pair it walks); pairs too selective for it get
+ * their cell's own launch over their rows, and pairs that outgrew the list are re-run on the bitmap walk of their
+ * cell, all on the device.  Other geometries, ef > 128 or ANNB_CELLS_GENERIC send every pair to its cell's own launch.
+ * A probed pair with fewer than k results gives ANNB_EFEWRESULTS.  At most ANNB_FILTER_MAX_PER_CALL distinct filters
+ * per cell (ANNB_ELIMIT).  Merge, outputs and parts as annb_cellset_search. */
+ANNB_API int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_space, int64_t B, int normalize,
+                              const int32_t *order, int n_probe, int limit, int ef, int flags, const int *query_filter,
+                              uint64_t *labels_out, float *dists_out, int32_t *cells_out, int out_space,
+                              uint64_t *part_labels, float *part_dists, int64_t *part_stats);
+/* What the last annb_cellset_search_prepared / annb_cellset_search_multi did besides the fused launch: (query, cell)
+ * pairs re-run on the bitmap walk, and cells served by their own filtered launch. */
 ANNB_API int annb_cellset_last_filtered(annb_cellset_t *cs, int64_t *rerun_pairs, int *handle_cells);
 ANNB_API int annb_cellset_merge(annb_cellset_t *cs, const uint64_t *labels, const float *dists, const int32_t *counts,
                        const int32_t *order, int in_space, int64_t B, int n_probe, int limit, uint64_t *labels_out,
@@ -425,7 +441,7 @@ ANNB_API int annb_cellset_merge(annb_cellset_t *cs, const uint64_t *labels, cons
 ANNB_API int annb_cellset_probe(annb_cellset_t *cs, const float *queries, int in_space, int64_t B, int n_probe,
                        int32_t *order_out, int out_space);
 /* Device time of the last probe / walk (fused launch, or the per-cell searches) / merge in ms, and the route the last
- * annb_cellset_search took (0 = fused walk, 1 = per-cell searches). */
+ * annb_cellset_search* call took (0 = fused walk, 1 = per-cell searches; annb_cellset_search_multi: own launches). */
 ANNB_API int annb_cellset_last_ms(annb_cellset_t *cs, float *probe_ms, float *walk_ms, float *merge_ms, int *route);
 
 /* ---- introspection for bench / roofline ------------------------------------------------------ */
