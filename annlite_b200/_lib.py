@@ -90,6 +90,8 @@ PROTOTYPES = {
     'annb_cellset_search_multi': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _int,
                                          _vp, _vp, _vp]),
     'annb_cellset_last_filtered': (_int, [_vp, C.POINTER(_i64), C.POINTER(_int)]),
+    'annb_cellset_set_bruteforce': (_int, [_vp, _vp]),
+    'annb_cellset_last_scanned': (_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
     'annb_cellset_merge': (_int, [_vp, _vp, _vp, _vp, _vp, _int, _i64, _int, _int, _vp, _vp, _vp, _int]),
     'annb_cellset_probe': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int]),
     'annb_cellset_last_ms': (_int, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(_int)]),

@@ -7,8 +7,10 @@ Differences from the reference, besides the docarray / SQLite / RocksDB stores i
 * a batch of queries runs as one GPU search (annb_cellset_search): without a filter or deletions, one launch builds
   each query's ADC table once and walks all its probed cells.  A dict filter or an id array is prepared on each probed
   cell and searched the same way with each cell's bitmap (annb_cellset_search_prepared), deletions included; a list
-  of per-query filter dicts too, each query with its own bitmap in each cell (annb_cellset_search_multi).  Cells with
-  `bruteforce_filter_below` set and unfiltered searches after deletions search the cells one by one.
+  of per-query filter dicts too, each query with its own bitmap in each cell (annb_cellset_search_multi).  A cell's
+  `bruteforce_filter_below`, read on every call, is passed along: a filter that admits at most that many of the cell's
+  rows is scanned exactly inside the same GPU search, as the cell's own search_batch would scan it.  Unfiltered
+  searches after deletions search the cells one by one.
 * equal distances in the merge keep concatenation order (the reference's argsort leaves them unspecified); a query
   with fewer than `limit` results is padded with +inf / UINT64_MAX / cell -1.
 * with a VQCodec attached, cells are probed in the order of annlite.math.cdist over the centroids.  The reference's
@@ -184,7 +186,7 @@ class CellContainer:
         per_query = is_per_query_filter(filter)
         if per_query and len(filter) != B:
             raise ValueError(f'{len(filter)} filters for {B} queries')
-        if not generic and all(v.bruteforce_filter_below is None for v in self._vec_indexes):
+        if not generic:
             if per_query:
                 return self._search_cells_multi(x, cells, filter, limit)
             return self._search_cells_prepared(x, cells, filter, limit)
@@ -226,10 +228,18 @@ class CellContainer:
         ol, od, oc = cs.merge(lab, dist, counts, cells, limit)
         return od, ol, oc
 
+    def _bruteforce_below(self):
+        """Each cell's current bruteforce_filter_below (-1 = none), or None when no cell sets one."""
+        below = [v.bruteforce_filter_below for v in self._vec_indexes]
+        if all(b is None for b in below):
+            return None
+        return np.array([-1 if b is None else int(b) for b in below], dtype=np.int64)
+
     def _search_cells_prepared(self, x, cells, filter, limit):
         """A dict filter or an id array over the probed cells in one GPU search (annb_cellset_search_prepared): the
         filter is prepared on each probed cell (an id array split by cell, each share prepared as a label list), and
-        every cell's k is what the per-cell route's search_batch uses: min(limit, live rows, admitted count)."""
+        every cell's k is what the per-cell route's search_batch uses: min(limit, live rows, admitted count).  A cell
+        whose filter admits at most its bruteforce_filter_below rows is scanned exactly, as search_batch scans it."""
         from .core.index.hnsw.index import PreparedFilter
         cs = self._cells()
         v0 = self._vec_indexes[0]
@@ -254,7 +264,7 @@ class CellContainer:
                     prepared.append(PreparedFilter(e, *e.filter_prepare_labels(mine.astype(np.uint64))))
                 fids[c] = prepared[-1].id
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
-                                       filter_ids=fids)
+                                       filter_ids=fids, bruteforce_below=self._bruteforce_below())
         finally:
             for p in prepared:
                 p.release()
@@ -264,7 +274,9 @@ class CellContainer:
         """One filter dict per query over the probed cells in one GPU search (annb_cellset_search_multi): the list is
         prepared on each probed cell with rows (HnswIndex.prepare_filters), whose ids form that cell's column of the
         (B, n_cells) table; every pair's k is what the per-cell route's search_batch uses: min(limit, live rows,
-        admitted count).  Cells not probed or empty keep a column of 0s (their k is 0 through the live count)."""
+        admitted count).  Cells not probed or empty keep a column of 0s (their k is 0 through the live count).  A pair
+        whose filter admits at most its cell's bruteforce_filter_below rows is scanned exactly, as _search_per_query
+        scans it."""
         cs = self._cells()
         v0 = self._vec_indexes[0]
         qids = np.zeros((x.shape[0], self.n_cells), dtype=np.int32)
@@ -276,7 +288,7 @@ class CellContainer:
                 prepared.append(self._vec_indexes[c].prepare_filters(filters))
                 qids[:, c] = prepared[-1].ids
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
-                                       query_filter_ids=qids)
+                                       query_filter_ids=qids, bruteforce_below=self._bruteforce_below())
         finally:
             for p in prepared:
                 p.release()

@@ -628,3 +628,325 @@ int launch_merge_topk(annb_index *h, const uint64_t *labels, const float *dists,
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;
 }
+
+// ---- the multi-subset exact scan (annb_cellset_search_prepared / _multi with bruteforce thresholds) -------------
+// A job is one subset of one cell (a prepared filter's admitted rows, or a label list's live entries) and the query rows
+// that scan it.  Gather: every job's subset is compacted (bitmap, in internal-id order, as annb_filter_labels lists it)
+// or read (id list, in order, repeats kept), and its code rows and labels are copied once from the cell's own-code array
+// into a contiguous scratch -- three launches for all jobs.  Scan: one launch for all jobs, a CTA per tile of one job's
+// queries.  k <= 16: scan_topk_tiled2's mapping (16 interleaved tables, a half-warp scores one row for 16 queries,
+// per-lane register lists, one CTA reduction); larger k: a warp per query with its table in shared memory and a
+// WarpList, as scan_topk_kernel.  The subset is never chunked, so each CTA's lists are final and go straight to the
+// pair's row of the by-cell scratch.  Arithmetic and order are K2's: d = sum_m T[m, code[m]] from 0.f in fp32, the k
+// best by (distance, position in the subset) -- annb_scan_subset's bits and order.
+namespace {
+
+constexpr int GATHER_THREADS = 256;  // one bitmap word (or one list entry) per thread
+constexpr int SCAN_WARP_TILE = 8;    // queries per CTA of the warp-per-query form
+
+// pass 1: admitted rows per block of a job's bitmap
+__global__ void __launch_bounds__(GATHER_THREADS) subset_count_kernel(const SubsetScan *__restrict__ jobs) {
+  const SubsetScan &J = jobs[blockIdx.y];
+  if (!J.bits) return;
+  const int64_t nb = (J.nwords + GATHER_THREADS - 1) / GATHER_THREADS;
+  if (blockIdx.x >= nb) return;
+  __shared__ unsigned int s;
+  if (threadIdx.x == 0) s = 0;
+  __syncthreads();
+  const int64_t w = (int64_t)blockIdx.x * GATHER_THREADS + threadIdx.x;
+  unsigned int c = w < J.nwords ? __popc(J.bits[w]) : 0u;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL_MASK, c, o);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s, c);
+  __syncthreads();
+  if (threadIdx.x == 0) J.block_offs[blockIdx.x] = s;
+}
+
+// pass 2: the block counts of each job's bitmap -> exclusive offsets (one thread per job: a few hundred blocks at most)
+__global__ void subset_offsets_kernel(const SubsetScan *__restrict__ jobs, int J) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= J || !jobs[j].bits) return;
+  const int64_t nb = (jobs[j].nwords + GATHER_THREADS - 1) / GATHER_THREADS;
+  unsigned int *o = jobs[j].block_offs;
+  unsigned int run = 0;
+  for (int64_t b = 0; b < nb; b++) {
+    const unsigned int c = o[b];
+    o[b] = run;
+    run += c;
+  }
+}
+
+// pass 3: each admitted row (bitmap, in id order) or list entry -> its code row and label at its subset position
+__global__ void __launch_bounds__(GATHER_THREADS) subset_gather_kernel(const SubsetScan *__restrict__ jobs) {
+  const SubsetScan &J = jobs[blockIdx.y];
+  const int64_t t = (int64_t)blockIdx.x * GATHER_THREADS + threadIdx.x;
+  if (!J.bits) {
+    if (blockIdx.x * (int64_t)GATHER_THREADS >= J.n) return;
+    if (t < J.n) {
+      const uint32_t id = J.ids[t];
+      reinterpret_cast<uint2 *>(J.codes)[t] = __ldg(reinterpret_cast<const uint2 *>(J.cell_codes) + id);
+      J.labels[t] = J.cell_labels[id];
+    }
+    return;
+  }
+  if (blockIdx.x * (int64_t)GATHER_THREADS >= J.nwords) return;
+  __shared__ unsigned int warp_sums[GATHER_THREADS / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint32_t word = t < J.nwords ? J.bits[t] : 0u;
+  const unsigned int c = __popc(word);
+  unsigned int x = c;  // inclusive scan over the warp, then over the warps
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int y = __shfl_up_sync(FULL_MASK, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sums[wid] = x;
+  __syncthreads();
+  unsigned int before = 0;
+  for (int w = 0; w < wid; w++) before += warp_sums[w];
+  int64_t pos = (int64_t)J.block_offs[blockIdx.x] + before + x - c;
+  while (word) {
+    const int b = __ffs(word) - 1;
+    word &= word - 1;
+    const int64_t id = t * 32 + b;
+    reinterpret_cast<uint2 *>(J.codes)[pos] = __ldg(reinterpret_cast<const uint2 *>(J.cell_codes) + id);
+    J.labels[pos] = J.cell_labels[id];
+    pos++;
+  }
+}
+
+// the k best of a pair -> its row of the by-cell scratch, found = k, counters {0 hops, 0 neighbours, n rows scored}
+__device__ __forceinline__ void subset_write_tail(const SubsetScan &J, int64_t row, int32_t *__restrict__ sfound,
+                                                  int64_t *__restrict__ sstats) {
+  sfound[row] = J.k;
+  if (sstats) {
+    sstats[row * 3 + 0] = 0;
+    sstats[row * 3 + 1] = 0;
+    sstats[row * 3 + 2] = J.n;
+  }
+}
+
+// tile i = (job, first query of the job); 16 queries per CTA, 16 warps
+template <int KK>
+__global__ void __launch_bounds__(TILED_WARPS * 32, 1)
+subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__restrict__ jobs, const int2 *__restrict__ tiles,
+                         int n_cells, int limit, uint64_t *__restrict__ sl, float *__restrict__ sd, int32_t *__restrict__ sfound,
+                         int64_t *__restrict__ sstats) {
+  constexpr int M = 8, KS = 256, TS = M * KS;
+  extern __shared__ float sT[];
+  __shared__ int64_t srow[QT];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int half = lane >> 4, q = lane & 15;
+  const int2 tile = tiles[blockIdx.x];
+  const SubsetScan &J = jobs[tile.x];
+  const int q0 = tile.y, nq = min(QT, J.nq - q0);
+  if (threadIdx.x < QT) srow[threadIdx.x] = threadIdx.x < nq ? (int64_t)J.queries[q0 + threadIdx.x] : -1;
+  __syncthreads();
+  for (int t = threadIdx.x; t < TS * QT; t += blockDim.x) {
+    const int qq = t & (QT - 1), i = t >> 4;
+    sT[t] = srow[qq] >= 0 ? __ldg(tables + srow[qq] * TS + i) : 0.f;
+  }
+  __syncthreads();
+  float Kd[KK];
+  uint32_t Ki[KK];
+#pragma unroll
+  for (int i = 0; i < KK; i++) {
+    Kd[i] = CUDART_INF_F;
+    Ki[i] = LIST_EMPTY_VAL;
+  }
+  const int64_t n = J.n;
+  const uint8_t *codes = J.codes;
+  const float *Tq = sT + q;
+  auto score = [&](const uint2 c) -> float {  // m sequential from 0.f, every add rounded (pq_bindings.pyx:30-47)
+    float d = 0.f;
+    d = __fadd_rn(d, Tq[((c.x & 0xffu) + 0 * KS) * QT]);
+    d = __fadd_rn(d, Tq[(((c.x >> 8) & 0xffu) + 1 * KS) * QT]);
+    d = __fadd_rn(d, Tq[(((c.x >> 16) & 0xffu) + 2 * KS) * QT]);
+    d = __fadd_rn(d, Tq[((c.x >> 24) + 3 * KS) * QT]);
+    d = __fadd_rn(d, Tq[((c.y & 0xffu) + 4 * KS) * QT]);
+    d = __fadd_rn(d, Tq[(((c.y >> 8) & 0xffu) + 5 * KS) * QT]);
+    d = __fadd_rn(d, Tq[(((c.y >> 16) & 0xffu) + 6 * KS) * QT]);
+    d = __fadd_rn(d, Tq[((c.y >> 24) + 7 * KS) * QT]);
+    return d;
+  };
+  constexpr int64_t STEP = 2 * TILED_WARPS;
+  int64_t r = 2 * warp + half;
+  for (; r + STEP < n; r += 2 * STEP) {
+    const uint2 ca = __ldg(reinterpret_cast<const uint2 *>(codes + r * 8));
+    const uint2 cb = __ldg(reinterpret_cast<const uint2 *>(codes + (r + STEP) * 8));
+    const float da = score(ca), db = score(cb);
+    lane_list_insert_ascending_rows<KK>(Kd, Ki, da, (uint32_t)r);
+    lane_list_insert_ascending_rows<KK>(Kd, Ki, db, (uint32_t)(r + STEP));
+  }
+  if (r < n) {
+    const uint2 ca = __ldg(reinterpret_cast<const uint2 *>(codes + r * 8));
+    lane_list_insert_ascending_rows<KK>(Kd, Ki, score(ca), (uint32_t)r);
+  }
+  // the odd-row half hands its list to the even-row half of the same query: (dist, position) order from here on
+#pragma unroll
+  for (int i = 0; i < KK; i++) {
+    const float od = __shfl_down_sync(FULL_MASK, Kd[i], 16);
+    const uint32_t oi = __shfl_down_sync(FULL_MASK, Ki[i], 16);
+    if (half == 0 && oi != LIST_EMPTY_VAL) lane_list_insert<KK>(Kd, Ki, od, oi);
+  }
+  // the 16 per-warp lists of a query -> one list, through the table area
+  __syncthreads();
+  float *rd = sT;
+  uint32_t *ri = reinterpret_cast<uint32_t *>(sT + QT * TILED_WARPS * KK);
+  if (half == 0) {
+#pragma unroll
+    for (int i = 0; i < KK; i++) {
+      rd[(q * TILED_WARPS + warp) * KK + i] = Kd[i];
+      ri[(q * TILED_WARPS + warp) * KK + i] = Ki[i];
+    }
+  }
+  __syncthreads();
+  // warp w finishes query w of the tile: lane l < 16 holds the list warp l produced
+#pragma unroll
+  for (int i = 0; i < KK; i++) {
+    Kd[i] = half == 0 ? rd[(warp * TILED_WARPS + q) * KK + i] : CUDART_INF_F;
+    Ki[i] = half == 0 ? ri[(warp * TILED_WARPS + q) * KK + i] : LIST_EMPTY_VAL;
+  }
+  if (warp >= nq) return;
+  const int64_t row = srow[warp] * n_cells + J.cell;
+  const int k = J.k;
+  for (int j = 0; j < k; j++) {
+    float md = Kd[0];
+    uint32_t mi = Ki[0];
+#pragma unroll
+    for (int s2 = 16; s2 > 0; s2 >>= 1) {
+      const float od = __shfl_xor_sync(FULL_MASK, md, s2);
+      const uint32_t oi = __shfl_xor_sync(FULL_MASK, mi, s2);
+      if (od < md || (od == md && oi < mi)) {
+        md = od;
+        mi = oi;
+      }
+    }
+    if (lane == 0) {
+      sd[row * limit + j] = md;
+      sl[row * limit + j] = mi == LIST_EMPTY_VAL ? UINT64_MAX : J.labels[mi];
+    }
+    if (Ki[0] == mi && mi != LIST_EMPTY_VAL) {  // positions are unique across the lists: exactly one lane pops its head
+#pragma unroll
+      for (int i = 0; i + 1 < KK; i++) {
+        Kd[i] = Kd[i + 1];
+        Ki[i] = Ki[i + 1];
+      }
+      Kd[KK - 1] = CUDART_INF_F;
+      Ki[KK - 1] = LIST_EMPTY_VAL;
+    }
+  }
+  if (lane == 0) subset_write_tail(J, row, sfound, sstats);
+}
+
+// k > 16: a warp per query (SCAN_WARP_TILE queries of one job per CTA), its table in shared memory, lanes over rows
+template <int EPL>
+__global__ void __launch_bounds__(SCAN_WARP_TILE * 32)
+subset_scan_warp_kernel(const float *__restrict__ tables, const SubsetScan *__restrict__ jobs, const int2 *__restrict__ tiles,
+                        int n_cells, int limit, uint64_t *__restrict__ sl, float *__restrict__ sd, int32_t *__restrict__ sfound,
+                        int64_t *__restrict__ sstats) {
+  constexpr int TS = 8 * 256;
+  extern __shared__ float sT[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int2 tile = tiles[blockIdx.x];
+  const SubsetScan &J = jobs[tile.x];
+  const int qi = tile.y + warp;
+  if (qi >= J.nq) return;
+  const int64_t qrow = J.queries[qi];
+  float *T = sT + warp * TS;
+  for (int i = lane; i < TS; i += 32) T[i] = __ldg(tables + qrow * TS + i);
+  __syncwarp();
+  const int k = J.k;
+  const int64_t n = J.n;
+  WarpList<EPL> L;
+  L.clear();
+  float worst = CUDART_INF_F;
+  for (int64_t base = 0; base < n; base += 32) {
+    const int64_t r = base + lane;
+    float d = CUDART_INF_F;
+    if (r < n) d = adc_lookup_u8x8(T, __ldg(reinterpret_cast<const uint2 *>(J.codes) + r), 256);
+    unsigned mask = __ballot_sync(FULL_MASK, d < worst);
+    while (mask) {
+      const int j = __ffs(mask) - 1;
+      mask &= mask - 1;
+      const float dj = __shfl_sync(FULL_MASK, d, j);
+      if (dj < worst) {
+        L.insert(dj, (uint32_t)(base + j), k);
+        worst = L.key_at(k - 1);
+      }
+    }
+  }
+  const int64_t row = qrow * n_cells + J.cell;
+#pragma unroll
+  for (int e = 0; e < EPL; e++) {
+    const int pos = e * 32 + lane;
+    if (pos < k) {
+      sd[row * limit + pos] = L.k[e];
+      sl[row * limit + pos] = L.v[e] == LIST_EMPTY_VAL ? UINT64_MAX : J.labels[L.v[e]];
+    }
+  }
+  if (lane == 0) subset_write_tail(J, row, sfound, sstats);
+}
+
+}  // namespace
+
+bool subset_scan_applicable(const annb_index *h) { return h->M == 8 && h->code_bytes == 1 && h->Ks == 256; }
+
+int subset_scan_tile_width(int kmax) { return kmax <= 16 ? QT : SCAN_WARP_TILE; }
+
+int launch_subset_scan(annb_index *h, cudaStream_t st, const SubsetScan *d_jobs, const std::vector<SubsetScan> &jobs,
+                       const int2 *d_tiles, int64_t n_tiles, const float *tables, int n_cells, int limit, uint64_t *sl,
+                       float *sd, int32_t *sfound, int64_t *sstats) {
+  const int J = (int)jobs.size();
+  if (J == 0 || n_tiles == 0) return ANNB_OK;
+  if (J > 65535) ANNB_FAIL(ANNB_ELIMIT, "%d subsets in one scan (limit 65535)", J);
+  int64_t gx = 1;
+  int kmax = 1;
+  bool any_bits = false;
+  for (const SubsetScan &s : jobs) {
+    gx = std::max(gx, s.bits ? (s.nwords + GATHER_THREADS - 1) / GATHER_THREADS : (s.n + GATHER_THREADS - 1) / GATHER_THREADS);
+    kmax = std::max(kmax, (int)s.k);
+    any_bits |= s.bits != nullptr;
+  }
+  if (kmax > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "k=%d exceeds ANNB_MAX_EF=%d", kmax, ANNB_MAX_EF);
+  const dim3 ggrid((unsigned)gx, (unsigned)J);
+  if (any_bits) {
+    subset_count_kernel<<<ggrid, GATHER_THREADS, 0, st>>>(d_jobs);
+    subset_offsets_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_jobs, J);
+    h->launches += 2;
+  }
+  subset_gather_kernel<<<ggrid, GATHER_THREADS, 0, st>>>(d_jobs);
+  h->launches++;
+  ANNB_CUDA(cudaGetLastError());
+  if (kmax <= 16) {
+    const size_t smem = (size_t)8 * 256 * QT * sizeof(float);
+#define SS_TILED(KKV)                                                                                                    \
+  {                                                                                                                      \
+    ANNB_CUDA(cudaFuncSetAttribute(subset_scan_tiled_kernel<KKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    subset_scan_tiled_kernel<KKV><<<(unsigned)n_tiles, TILED_WARPS * 32, smem, st>>>(tables, d_jobs, d_tiles, n_cells, limit, sl, sd, \
+                                                                                   sfound, sstats);                    \
+  }
+    if (kmax <= 1) SS_TILED(1)
+    else if (kmax <= 10) SS_TILED(10)
+    else SS_TILED(16)
+#undef SS_TILED
+  } else {
+    const size_t smem = (size_t)SCAN_WARP_TILE * 8 * 256 * sizeof(float);
+#define SS_WARP(E)                                                                                                       \
+  {                                                                                                                      \
+    ANNB_CUDA(cudaFuncSetAttribute(subset_scan_warp_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    subset_scan_warp_kernel<E><<<(unsigned)n_tiles, SCAN_WARP_TILE * 32, smem, st>>>(tables, d_jobs, d_tiles, n_cells, limit, sl, sd, \
+                                                                                   sfound, sstats);                    \
+  }
+    const int epl = (kmax + 31) / 32;
+    if (epl <= 1) SS_WARP(1)
+    else if (epl <= 2) SS_WARP(2)
+    else if (epl <= 4) SS_WARP(4)
+    else if (epl <= 8) SS_WARP(8)
+    else SS_WARP(16)
+#undef SS_WARP
+  }
+  h->launches++;
+  ANNB_CUDA(cudaGetLastError());
+  return ANNB_OK;
+}

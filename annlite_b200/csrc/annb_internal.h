@@ -189,6 +189,28 @@ struct PreparedFilter {
   int64_t n = 0;             // rows it covers (gd.n at prepare time)
   int64_t count = 0;         // admitted rows
   uint64_t gen = 0;          // annb_index::state_gen at prepare time
+  // a label-prepared filter (annb_filter_prepare_labels): the list's entries that name live rows, as internal ids in
+  // the caller's order with repeats kept (what annb_scan_subset scans for that list); nullptr for a program's filter
+  const uint32_t *ids = nullptr;
+  int64_t n_ids = 0;
+};
+
+// One subset of a cell scanned exactly for some of the batch's queries (the multi-subset scan, adc_scan.cu).  The
+// subset is a bitmap by internal id, compacted in id order (the order annb_filter_labels lists it), or a list of
+// internal ids; its code rows and labels are gathered once into `codes` / `labels`.  Each query row in `queries` gets
+// the k best (distance, position in the subset) in its pair's row (q * n_cells + cell) of the by-cell scratch.
+struct SubsetScan {
+  const uint32_t *bits;        // bitmap by internal id, or nullptr
+  const uint32_t *ids;         // when bits == nullptr: internal ids in order
+  int64_t nwords;              // bitmap words to compact
+  const uint8_t *cell_codes;   // the cell's (rows, 8) own codes by internal id
+  const uint64_t *cell_labels; // the cell's labels by internal id
+  uint8_t *codes;              // gathered (n, 8) code rows
+  uint64_t *labels;            // gathered labels
+  unsigned int *block_offs;    // bitmap: per-block counts, then offsets
+  int64_t n;                   // subset rows
+  const uint32_t *queries;     // query rows that scan the subset
+  int32_t nq, k, cell, pad;
 };
 
 // a batch with one filter per query (annb_search_multi / annb_search_submit_multi), in its gathered row order: the
@@ -245,6 +267,10 @@ struct annb_index {
   uint64_t *d_labels = nullptr;
   uint32_t *d_deleted = nullptr;
   size_t cap_rec0 = 0, cap_up = 0, cap_labels = 0, cap_deleted = 0;
+  // every node's own code (n, code_row) by internal id, for the exact subset scan; built on first use per state_gen
+  uint8_t *d_own_codes = nullptr;
+  size_t cap_own_codes = 0;
+  uint64_t own_codes_gen = 0;
 
   // scratch (grown on demand)
   void *d_scratch[40] = {nullptr};
@@ -353,6 +379,16 @@ int launch_walk4f_cells(annb_index *h, const SearchParams &p, int ep, int en);
 int find_prepared_filter(annb_index *h, int filter_id, PreparedFilter **out);
 int search_prepared_stats(annb_index *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef, int filter_id,
                           uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out);
+// the handle's own-code array (annb_index::d_own_codes), current for the graph as it is now (caller holds the lock)
+int sync_own_codes(annb_index *h, const uint8_t **out);
+// the multi-subset exact scan (adc_scan.cu) over J jobs (d_jobs on the device, `jobs` its host copy): gather every
+// subset's rows, then score every job's queries against its subset with the batch's K1 tables (B, 8, 256), k <= 512,
+// results straight into the by-cell scratch (found = k, counters {0, 0, n}); M = 8 one-byte codes, Ks = 256 only
+bool subset_scan_applicable(const annb_index *h);
+int subset_scan_tile_width(int kmax);
+int launch_subset_scan(annb_index *h, cudaStream_t st, const SubsetScan *d_jobs, const std::vector<SubsetScan> &jobs,
+                       const int2 *d_tiles, int64_t n_tiles, const float *tables, int n_cells, int limit, uint64_t *sl,
+                       float *sd, int32_t *sfound, int64_t *sstats);
 // G ascending (dist, label) lists of k per query -> global k best; *_gstride = distance between two shards' arrays in elements
 int launch_merge_topk(annb_index *h, const uint64_t *labels, const float *dists, int G, int64_t B, int k, int64_t l_gstride,
                       int64_t d_gstride, uint64_t *labels_out, float *dists_out, cudaStream_t stream);

@@ -191,6 +191,7 @@ int annb_destroy(annb_index_t *h) {
   if (h->d_up) cudaFree(h->d_up);
   if (h->d_labels) cudaFree(h->d_labels);
   if (h->d_deleted) cudaFree(h->d_deleted);
+  if (h->d_own_codes) cudaFree(h->d_own_codes);
   for (AttrColumn &c : h->attrs) {
     if (c.d_vals) cudaFree(c.d_vals);
     if (c.d_valid) cudaFree(c.d_valid);
@@ -1887,6 +1888,23 @@ static int prepare_many_impl(annb_index *h, int F, const annb_filter_op_t *progr
 // the cell sets (cells.cu) use a cell's prepared filters under that cell's lock
 int find_prepared_filter(annb_index *h, int filter_id, PreparedFilter **out) { return find_filter(h, filter_id, out); }
 
+// The walk layout keeps a node's code only in its neighbours' records; the exact subset scan reads each node's own code
+// from this copy of the host graph's, re-made after any change (state_gen) on the first scan that needs it.
+int sync_own_codes(annb_index *h, const uint8_t **out) {
+  HostGraph &g = h->g;
+  const int64_t n = g.count.load();
+  const size_t crow = g.code_row_bytes;
+  if (!h->d_own_codes || h->own_codes_gen != h->state_gen) {
+    std::vector<uint8_t> hc((size_t)n * crow);
+    for (int64_t i = 0; i < n; i++) memcpy(hc.data() + (size_t)i * crow, g.code((uint32_t)i), crow);
+    ANNB_TRY(ensure_dev((void **)&h->d_own_codes, &h->cap_own_codes, std::max<size_t>(hc.size(), 16)));
+    if (n) ANNB_CUDA(cudaMemcpy(h->d_own_codes, hc.data(), hc.size(), cudaMemcpyHostToDevice));
+    h->own_codes_gen = h->state_gen;
+  }
+  *out = h->d_own_codes;
+  return ANNB_OK;
+}
+
 // annb_search_prepared with the (B, 3) counters of annb_search; takes the handle's lock
 int search_prepared_stats(annb_index *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef, int filter_id,
                           uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out) {
@@ -2030,11 +2048,25 @@ int annb_filter_prepare_labels(annb_index_t *h, const uint64_t *labels, int64_t 
   ANNB_TRY(sync_device_graph(h));
   const int64_t rows = h->gd.n;
   const size_t words = (size_t)(rows + 31) / 32 + 1;
+  // the entries that name live rows, in order, repeats kept: the subset an exact scan of this list covers
+  std::vector<uint64_t> hl;
+  const uint64_t *lab = labels;
+  if (space == ANNB_DEVICE && n > 0) {
+    hl.resize((size_t)n);
+    ANNB_CUDA(cudaMemcpy(hl.data(), labels, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    lab = hl.data();
+  }
+  std::vector<uint32_t> ids;
+  for (int64_t i = 0; i < n; i++) {
+    auto it = h->g.label_lookup.find(lab[i]);
+    if (it != h->g.label_lookup.end() && !h->g.deleted(it->second)) ids.push_back(it->second);
+  }
   void *block = nullptr;
-  ANNB_CUDA(cudaMalloc(&block, words * 4));
+  ANNB_CUDA(cudaMalloc(&block, (words + ids.size()) * 4));
   std::shared_ptr<void> owner(block, [](void *p) { cudaFree(p); });
   uint32_t *bits = (uint32_t *)block;
   ANNB_CUDA(cudaMemsetAsync(bits, 0, words * 4, h->stream));
+  if (!ids.empty()) ANNB_CUDA(cudaMemcpyAsync(bits + words, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, h->stream));
   ANNB_TRY(labels_to_bitmap(h, labels, space, n, bits));
   ANNB_CUDA(cudaStreamSynchronize(h->stream));
   PreparedFilter pf;
@@ -2043,6 +2075,8 @@ int annb_filter_prepare_labels(annb_index_t *h, const uint64_t *labels, int64_t 
   pf.n = rows;
   pf.count = n;  // as a label list counts: every entry, repeats and labels not in the graph included
   pf.gen = h->state_gen;
+  pf.ids = bits + words;
+  pf.n_ids = (int64_t)ids.size();
   const int id = h->next_filter_id++;
   h->filters[id] = pf;
   *filter_id = id;

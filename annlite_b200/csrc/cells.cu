@@ -28,13 +28,17 @@ struct annb_cellset {
   int last_route = 0;
   int64_t last_rerun_pairs = 0;     // annb_cellset_search_prepared / _multi: (query, cell) pairs re-run on the bitmap walk
   int last_handle_cells = 0;        // ... and cells served by their own filtered launch instead of the fused walk
+  std::vector<int64_t> below;       // annb_cellset_set_bruteforce: per cell, scan filters admitting <= this many (-1 = never)
+  int64_t last_scanned_pairs = 0;   // (query, cell) pairs the last filtered search scanned exactly ...
+  int64_t last_scanned_rows = 0;    // ... and the rows those scans scored
 };
 
 namespace {
 
 enum { C_QUERIES = 0, C_ORDER, C_K, C_LABELS, C_DISTS, C_FOUND, C_STATS, C_OUT, C_BITS, C_TABLES, C_TMP_L, C_TMP_D, C_TMP_F,
-       C_TMP_S, C_QMAP, C_SLOT, C_SLOT_K, C_SLOT_BITS, C_GTABLES, C_QF };
-static_assert(C_QF < 24, "annb_cellset::buf is too small");
+       C_TMP_S, C_QMAP, C_SLOT, C_SLOT_K, C_SLOT_BITS, C_GTABLES, C_QF, C_SCAN_JOBS, C_SCAN_ROWS, C_SCAN_QUERIES,
+       C_SCAN_BLOCKS };
+static_assert(C_SCAN_BLOCKS < 24, "annb_cellset::buf is too small");
 
 int cs_buf(annb_cellset *cs, int slot, size_t bytes, void **out) {
   if (bytes == 0) bytes = 16;
@@ -409,6 +413,132 @@ int merge_and_finish(annb_cellset *cs, const float *sd, const uint64_t *sl, cons
   return ANNB_OK;
 }
 
+// One exact subset scan of a filtered cell-set search: cell `cell`'s prepared filter `f` (its admitted rows in id
+// order, or a label list's live entries in order) scanned for the query rows `rows` with k results each.
+struct ScanPlan {
+  int cell = 0, k = 0;
+  const PreparedFilter *f = nullptr;
+  std::vector<uint32_t> rows;
+};
+
+int64_t plan_rows(const ScanPlan &p) { return p.f->ids ? p.f->n_ids : p.f->count; }
+
+// a scanned pair with fewer live subset entries than its k fails as annb_scan_subset fails
+int check_plans(const std::vector<ScanPlan> &plans) {
+  for (const ScanPlan &p : plans)
+    if (!p.rows.empty() && plan_rows(p) < p.k)
+      ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+  return ANNB_OK;
+}
+
+// The scans of a search, uploaded: the job table, the query rows and tiles, and the launch groups
+struct StagedScans {
+  std::vector<SubsetScan> jobs;
+  std::vector<std::pair<size_t, size_t>> groups;  // [first, last) jobs of each launch
+  std::vector<int64_t> tile0;                     // first tile of each launch (+ the end)
+  SubsetScan *djobs = nullptr;
+  int2 *dtiles = nullptr;
+};
+
+// The plans (in cell order) staged on the cell set's stream, before the walk: one gather and one scan for all plans, or
+// (per_cell) for each cell's plans in turn.  Counts the scanned pairs and rows.
+int stage_scans(annb_cellset *cs, const std::vector<ScanPlan> &plans, const std::vector<const uint8_t *> &own,
+                const std::vector<GraphDev> &gd, bool per_cell, StagedScans &ss) {
+  const size_t J = plans.size();
+  if (J == 0) return ANNB_OK;
+  cudaStream_t st = cs->h0->stream;
+  int64_t rows = 0, blocks = 0, nq = 0;
+  for (const ScanPlan &p : plans) {
+    rows += plan_rows(p);
+    if (!p.f->ids) blocks += ((p.f->n + 31) / 32 + 255) / 256;
+    nq += (int64_t)p.rows.size();
+  }
+  // launch groups: [g0, g1) ranges of plans, each with its tiles
+  std::vector<std::pair<size_t, size_t>> &groups = ss.groups;
+  for (size_t j = 0; j < J; j++)
+    if (groups.empty() || (per_cell && plans[j].cell != plans[groups.back().first].cell)) groups.push_back({j, j + 1});
+    else groups.back().second = j + 1;
+  std::vector<int2> tiles;
+  std::vector<int64_t> &tile0 = ss.tile0;
+  for (auto &g : groups) {
+    int kmax = 1;
+    for (size_t j = g.first; j < g.second; j++) kmax = std::max(kmax, plans[j].k);
+    const int w = subset_scan_tile_width(kmax);
+    tile0.push_back((int64_t)tiles.size());
+    for (size_t j = g.first; j < g.second; j++)
+      for (size_t q0 = 0; q0 < plans[j].rows.size(); q0 += (size_t)w) tiles.push_back(make_int2((int)(j - g.first), (int)q0));
+  }
+  tile0.push_back((int64_t)tiles.size());
+  uint64_t *glab;
+  uint32_t *dq;
+  unsigned int *boffs;
+  SubsetScan *djobs;
+  const size_t qwords = ((size_t)nq + 1) / 2 * 2;
+  ANNB_TRY_RC(cs_buf(cs, C_SCAN_ROWS, (size_t)rows * 16, (void **)&glab));
+  ANNB_TRY_RC(cs_buf(cs, C_SCAN_QUERIES, qwords * 4 + tiles.size() * sizeof(int2), (void **)&dq));
+  ANNB_TRY_RC(cs_buf(cs, C_SCAN_BLOCKS, (size_t)blocks * 4, (void **)&boffs));
+  ANNB_TRY_RC(cs_buf(cs, C_SCAN_JOBS, J * sizeof(SubsetScan), (void **)&djobs));
+  int2 *dtiles = reinterpret_cast<int2 *>(dq + qwords);
+  uint8_t *gcodes = reinterpret_cast<uint8_t *>(glab + rows);
+  std::vector<SubsetScan> &jobs = ss.jobs;
+  jobs.resize(J);
+  std::vector<uint32_t> hq;
+  hq.reserve((size_t)nq);
+  int64_t r0 = 0, bl0 = 0;
+  for (size_t j = 0; j < J; j++) {
+    const ScanPlan &p = plans[j];
+    SubsetScan &s = jobs[j];
+    memset(&s, 0, sizeof(s));
+    s.bits = p.f->ids ? nullptr : p.f->bits;
+    s.ids = p.f->ids;
+    s.nwords = (p.f->n + 31) / 32;
+    s.cell_codes = own[p.cell];
+    s.cell_labels = gd[p.cell].labels;
+    s.codes = gcodes + r0 * 8;
+    s.labels = glab + r0;
+    s.block_offs = boffs + bl0;
+    s.n = plan_rows(p);
+    s.queries = dq + hq.size();
+    s.nq = (int32_t)p.rows.size();
+    s.k = p.k;
+    s.cell = p.cell;
+    r0 += s.n;
+    if (s.bits) bl0 += (s.nwords + 255) / 256;
+    hq.insert(hq.end(), p.rows.begin(), p.rows.end());
+    cs->last_scanned_pairs += s.nq;
+    cs->last_scanned_rows += (int64_t)s.nq * s.n;
+  }
+  ANNB_CUDA(cudaMemcpyAsync(djobs, jobs.data(), J * sizeof(SubsetScan), cudaMemcpyHostToDevice, st));
+  ANNB_CUDA(cudaMemcpyAsync(dq, hq.data(), hq.size() * 4, cudaMemcpyHostToDevice, st));
+  ANNB_CUDA(cudaMemcpyAsync(dtiles, tiles.data(), tiles.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+  ss.djobs = djobs;
+  ss.dtiles = dtiles;
+  return ANNB_OK;  // (pageable sources: each copy has taken its data when it returns)
+}
+
+// the staged scans, after the fused walk (which writes the rows of the pairs it skips): results into the by-cell scratch
+int launch_scans(annb_cellset *cs, const StagedScans &ss, const float *tables, const Staged &b, int limit) {
+  for (size_t g = 0; g < ss.groups.size(); g++) {
+    const size_t j0 = ss.groups[g].first, j1 = ss.groups[g].second;
+    const std::vector<SubsetScan> part(ss.jobs.begin() + (ptrdiff_t)j0, ss.jobs.begin() + (ptrdiff_t)j1);
+    ANNB_TRY_RC(launch_subset_scan(cs->h0, cs->h0->stream, ss.djobs + j0, part, ss.dtiles + ss.tile0[g], ss.tile0[g + 1] - ss.tile0[g],
+                                   tables, cs->n_cells, limit, b.sl, b.sd, b.sfound, b.sstats));
+  }
+  return ANNB_OK;
+}
+
+// cell c's filter `f` is scanned rather than walked: its threshold is set and the filter admits at most that many
+// (`need_rows`: and at least one); the scan's geometry and the cell's own codes are checked / made current here
+int scan_decision(annb_cellset *cs, int c, const PreparedFilter *f, bool need_rows, std::vector<const uint8_t *> &own, bool *out) {
+  const int64_t lim = cs->below.empty() ? -1 : cs->below[(size_t)c];
+  *out = lim >= 0 && f->count <= lim && (!need_rows || f->count > 0);
+  if (!*out || own[(size_t)c]) return ANNB_OK;
+  annb_index *h = cs->cells[(size_t)c];
+  if (!subset_scan_applicable(h))
+    ANNB_FAIL(ANNB_ELIMIT, "cell %d: the exact subset scan needs M = 8 one-byte codes with 256 centroids", c);
+  return sync_own_codes(h, &own[(size_t)c]);
+}
+
 }  // namespace
 
 extern "C" {
@@ -564,6 +694,9 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
   std::vector<int32_t> kc(C, 0);
   std::vector<const uint32_t *> bits(C, nullptr);
   std::vector<float> sel(C, 0.f);
+  std::vector<const PreparedFilter *> pfs(C, nullptr);
+  std::vector<char> scan(C, 0);  // 1 = the cell's subset is scanned exactly (annb_cellset_set_bruteforce)
+  std::vector<const uint8_t *> own_codes(C, nullptr);
   bool fused = !(flags & ANNB_CELLS_GENERIC);
   for (int c = 0; c < C; c++) {
     annb_index *h = cs->cells[c];
@@ -585,6 +718,10 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       bits[c] = f->bits;
       // the selectivity annb_search_prepared sizes the cell's lists by (SearchParams::selectivity is fp32)
       sel[c] = (float)std::min<double>(1.0, (double)f->count / (double)std::max<int64_t>(1, h->gd.n));
+      pfs[c] = f;
+      bool sc;
+      ANNB_TRY_RC(scan_decision(cs, c, f, true, own_codes, &sc));
+      scan[c] = sc;
     }
     int ep, en;
     fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
@@ -594,7 +731,7 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
   int ep = ef_max <= 64 ? 2 : 4, en = 0, n_own = 0;
   if (fused) {
     for (int c = 0; c < C; c++) {
-      if (kc[c] == 0) continue;
+      if (kc[c] == 0 || scan[c]) continue;
       int ep_c, en_c;
       if (walk4f_geometry(cs->cells[c], std::max(ef, kc[c]), (double)sel[c], &ep_c, &en_c)) {
         en = std::max(en, en_c);
@@ -608,24 +745,71 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
   cs->last_route = fused ? 0 : 1;
   cs->last_rerun_pairs = 0;
   cs->last_handle_cells = 0;
+  cs->last_scanned_pairs = 0;
+  cs->last_scanned_rows = 0;
   if (B == 0) return ANNB_OK;
   cudaStream_t st = h0->stream;
   Staged b;
   ANNB_TRY_RC(stage_batch(cs, queries, in_space, B, order, n_probe, limit, part_stats != nullptr, b));
   std::vector<int32_t> hfound;
   int64_t reruns = 0;
+  // the scanned cells: every query that probes one scans its subset with k_c (annb_scan_subset over the whole batch in
+  // the per-cell route; the merge reads only the probing queries' rows)
+  std::vector<ScanPlan> plans;
+  bool any_scan = false;
+  for (int c = 0; c < C; c++) any_scan |= scan[c] && kc[c] > 0;
+  if (any_scan) {
+    std::vector<int32_t> otmp;
+    const int32_t *ho;
+    ANNB_TRY_RC(host_order(cs, order, in_space, b.dorder, B, n_probe, otmp, &ho));
+    std::vector<int> at(C, -1);
+    for (int c = 0; c < C; c++)
+      if (scan[c] && kc[c] > 0) {
+        at[c] = (int)plans.size();
+        plans.emplace_back();
+        plans.back().cell = c;
+        plans.back().k = kc[c];
+        plans.back().f = pfs[c];
+      }
+    for (int64_t q = 0; q < B; q++)
+      for (int i = 0; i < n_probe; i++) {
+        const int c = ho[q * n_probe + i];
+        if (at[c] >= 0) plans[(size_t)at[c]].rows.push_back((uint32_t)q);
+      }
+    ANNB_TRY_RC(check_plans(plans));
+  }
+  // the K1 tables of the whole batch, for the scans, the cells' own launches and the re-runs (built once)
+  float *tables = nullptr;
+  auto need_tables = [&]() -> int {
+    if (tables) return ANNB_OK;
+    ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * h0->M * h0->Ks * sizeof(float), (void **)&tables));
+    std::lock_guard<std::mutex> lk(h0->mu);
+    return launch_adc_table(h0, b.dq, B, tables);
+  };
   if (!fused) {
-    // one annb_search_prepared per probed cell; a walk with fewer than k_c results fails the call as it fails the cell
-    ANNB_TRY_RC(per_cell_route(cs, order, in_space, b.dorder, B, n_probe, limit, kc, b.sl, b.sd, b.sfound, b.sstats,
+    // one annb_search_prepared per probed cell that is not scanned; a walk with fewer than k_c results fails the call as
+    // it fails the cell
+    std::vector<int32_t> kpc(kc);
+    for (int c = 0; c < C; c++)
+      if (scan[c]) kpc[c] = 0;
+    ANNB_TRY_RC(per_cell_route(cs, order, in_space, b.dorder, B, n_probe, limit, kpc, b.sl, b.sd, b.sfound, b.sstats,
                                [&](int c, int k, uint64_t *hl, float *hd, int64_t *hs) {
                                  return search_prepared_stats(cs->cells[c], queries, in_space, B, normalize, k, ef, filter_ids[c],
                                                               hl, hd, ANNB_HOST, hs);
                                }));
+    if (!plans.empty()) {  // one scan launch per scanned cell, on the device
+      for (int r = 0; r < normalize; r++) ANNB_TRY_RC(launch_l2_normalize(h0, b.dq, B, cs->dim));
+      StagedScans ss;
+      ANNB_TRY_RC(stage_scans(cs, plans, own_codes, gd, true, ss));
+      ANNB_TRY_RC(need_tables());
+      ANNB_TRY_RC(launch_scans(cs, ss, tables, b, limit));
+      cudaEventRecord(cs->ev[3], st);
+    }
   } else {
     for (int r = 0; r < normalize; r++) ANNB_TRY_RC(launch_l2_normalize(h0, b.dq, B, cs->dim));
     std::vector<int32_t> kwalk(kc);
     for (int c = 0; c < C; c++)
-      if (own[c]) kwalk[c] = 0;
+      if (own[c] || scan[c]) kwalk[c] = 0;
     int32_t *dk;
     const uint32_t **dbits;
     ANNB_TRY_RC(cs_buf(cs, C_K, (size_t)C * 4, (void **)&dk));
@@ -636,6 +820,9 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
     std::vector<int32_t> otmp;
     const int32_t *ho;
     ANNB_TRY_RC(host_order(cs, order, in_space, b.dorder, B, n_probe, otmp, &ho));
+    StagedScans ss;
+    ANNB_TRY_RC(stage_scans(cs, plans, own_codes, gd, false, ss));
+    if (!plans.empty()) ANNB_TRY_RC(need_tables());
     cudaEventRecord(cs->ev[2], st);
     if (en > 0) {
       SearchParams p;
@@ -646,14 +833,8 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       if (rc == 1) ANNB_FAIL(ANNB_ESTATE, "the filtered multi-cell walk does not apply to these cells");
       if (rc) return rc;
     }
-    // the K1 tables of the whole batch, for the cells' own launches and the re-runs (built once)
-    float *tables = nullptr;
-    auto need_tables = [&]() -> int {
-      if (tables) return ANNB_OK;
-      ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * h0->M * h0->Ks * sizeof(float), (void **)&tables));
-      std::lock_guard<std::mutex> lk(h0->mu);
-      return launch_adc_table(h0, b.dq, B, tables);
-    };
+    // the scans, one launch for every scanned cell
+    if (!plans.empty()) ANNB_TRY_RC(launch_scans(cs, ss, tables, b, limit));
     // one filtered launch of cell c on its own handle's stream (after everything queued on the cell set's, which waits
     // for it in turn): rows idx (n of them, or every row) of a (B, k_c) output, scattered into the cell's scratch rows
     auto cell_launch = [&](int c, int mode, const uint32_t *idx, int64_t n) -> int {
@@ -705,7 +886,7 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
     std::vector<std::vector<uint32_t>> over(C);
     std::vector<char> walked((size_t)B * C, 0);
     for (int64_t q = 0; q < B; q++) {
-      for (int i = 0; i < n_probe; i++) walked[q * C + ho[q * n_probe + i]] = 1;
+      for (int i = 0; i < n_probe; i++) walked[q * C + ho[q * n_probe + i]] = !scan[ho[q * n_probe + i]];
       for (int c = 0; c < C; c++) {
         if (own[c] && probed[c]) walked[q * C + c] = 1;
         if (walked[q * C + c] && hfound[q * C + c] < 0) over[c].push_back((uint32_t)q);
@@ -782,6 +963,9 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
   std::vector<int32_t> sk((size_t)(S * C), 0);
   std::vector<const uint32_t *> sbits((size_t)(S * C), nullptr);  // nullptr = no filter in this cell
   std::vector<float> ssel((size_t)(S * C), 1.f);
+  std::vector<const PreparedFilter *> spf((size_t)(S * C), nullptr);
+  std::vector<char> sscan((size_t)(S * C), 0);  // 1 = the pair's subset is scanned exactly (annb_cellset_set_bruteforce)
+  std::vector<const uint8_t *> own_codes(C, nullptr);
   bool fused = !(flags & ANNB_CELLS_GENERIC);
   for (int c = 0; c < C; c++) {
     annb_index *h = cs->cells[c];
@@ -819,6 +1003,10 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       sk[i] = (int32_t)std::min<int64_t>({(int64_t)limit, f->count, live});
       sbits[i] = f->bits;
       ssel[i] = (float)std::min<double>(1.0, (double)f->count / nn);
+      spf[i] = f;
+      bool sc;
+      ANNB_TRY_RC(scan_decision(cs, c, f, false, own_codes, &sc));
+      sscan[i] = sc;
     }
     int ep, en;
     fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
@@ -826,6 +1014,8 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
   cs->last_route = fused ? 0 : 1;
   cs->last_rerun_pairs = 0;
   cs->last_handle_cells = 0;
+  cs->last_scanned_pairs = 0;
+  cs->last_scanned_rows = 0;
   if (B == 0) return ANNB_OK;
   cudaStream_t st = h0->stream;
   Staged b;
@@ -834,27 +1024,51 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
   std::vector<int32_t> otmp;
   const int32_t *ho;
   ANNB_TRY_RC(host_order(cs, order, in_space, b.dorder, B, n_probe, otmp, &ho));
-  // the pairs walked: probed, with k > 0 (and which slots probe which cells)
+  // the pairs walked: probed, with k > 0, not scanned (and which slots probe which cells); the scanned ones: one plan per
+  // (cell, filter), its queries in batch order
   std::vector<char> walked((size_t)(B * C), 0), sprobed((size_t)(S * C), 0);
+  std::map<std::pair<int, int>, ScanPlan> by_filter;
   for (int64_t q = 0; q < B; q++)
     for (int i = 0; i < n_probe; i++) {
       const int c = ho[q * n_probe + i];
       const size_t sc = (size_t)slot[(size_t)q] * C + c;
       sprobed[sc] = 1;
-      walked[(size_t)(q * C + c)] = sk[sc] > 0;
+      walked[(size_t)(q * C + c)] = sk[sc] > 0 && !sscan[sc];
+      if (sk[sc] > 0 && sscan[sc]) {
+        ScanPlan &pl = by_filter[{c, row_id(slot[(size_t)q], c)}];
+        pl.cell = c;
+        pl.k = sk[sc];
+        pl.f = spf[sc];
+        pl.rows.push_back((uint32_t)q);
+      }
     }
+  std::vector<ScanPlan> plans;
+  for (auto &kv : by_filter) plans.push_back(std::move(kv.second));
+  ANNB_TRY_RC(check_plans(plans));
   // fused route: the pairs hnsw_walk4f serves, and N's size (the largest any of them needs alone)
   std::vector<char> own((size_t)(S * C), 0);  // 1 = the pair goes to its cell's own launch
   int ep = ef_max <= 64 ? 2 : 4, en = 0;
   for (int64_t s = 0; s < S; s++)
     for (int c = 0; c < C; c++) {
       const size_t i = (size_t)(s * C + c);
-      if (!sprobed[i] || sk[i] == 0) continue;
+      if (!sprobed[i] || sk[i] == 0 || sscan[i]) continue;
       int ep_c, en_c;
       if (fused && walk4f_geometry(cs->cells[c], std::max(ef, sk[i]), (double)ssel[i], &ep_c, &en_c)) en = std::max(en, en_c);
       else own[i] = 1;
     }
   if (ep == 4 && en > 0) en = en <= 4 ? 4 : (en <= 6 ? 6 : 8);
+  // the K1 tables of the whole batch, for the scans, the own launches and the re-runs (built once)
+  const int TS = h0->M * h0->Ks;
+  float *tables = nullptr;
+  auto need_tables = [&]() -> int {
+    if (tables) return ANNB_OK;
+    ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * TS * sizeof(float), (void **)&tables));
+    std::lock_guard<std::mutex> lk(h0->mu);
+    return launch_adc_table(h0, b.dq, B, tables);
+  };
+  StagedScans ss;
+  ANNB_TRY_RC(stage_scans(cs, plans, own_codes, gd, !fused, ss));
+  if (!plans.empty()) ANNB_TRY_RC(need_tables());
   cudaEventRecord(cs->ev[2], st);
   if (en > 0) {
     // the walk's tables: k per (slot, cell) (0 = skip, own-launch pairs included) and the admission word: the filter's
@@ -863,7 +1077,7 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
     std::vector<uintptr_t> word((size_t)(S * C));
     for (size_t i = 0; i < word.size(); i++) {
       const int c = (int)(i % C);
-      if (own[i]) kwalk[i] = 0;
+      if (own[i] || sscan[i]) kwalk[i] = 0;
       const uint32_t *bits = sbits[i] ? sbits[i] : gd[c].deleted;  // (sync_device_graph always uploads the deletions)
       if (kwalk[i] > 0 && (!bits || (reinterpret_cast<uintptr_t>(bits) & 3u)))
         ANNB_FAIL(ANNB_ESTATE, "internal: cell %d has no 4-byte aligned admission bitmap", c);
@@ -887,15 +1101,8 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
     if (rc == 1) ANNB_FAIL(ANNB_ESTATE, "the per-query filtered multi-cell walk does not apply to these cells");
     if (rc) return rc;
   }
-  // the K1 tables of the whole batch, for the own launches and the re-runs (built once)
-  const int TS = h0->M * h0->Ks;
-  float *tables = nullptr;
-  auto need_tables = [&]() -> int {
-    if (tables) return ANNB_OK;
-    ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * TS * sizeof(float), (void **)&tables));
-    std::lock_guard<std::mutex> lk(h0->mu);
-    return launch_adc_table(h0, b.dq, B, tables);
-  };
+  // the scans, after the walk: one launch for all of them (ANNB_CELLS_GENERIC / other geometries: one per cell)
+  if (!plans.empty()) ANNB_TRY_RC(launch_scans(cs, ss, tables, b, limit));
   // one launch of cell c over query rows `rows` (their tables gathered) with k, on its own handle's stream (after
   // everything queued on the cell set's, which waits for it in turn); `qf` = each row's bitmap (nullptr = no filter),
   // or empty for a launch without per-query filters; its outputs scattered into the rows' pairs of the scratch
@@ -1077,6 +1284,23 @@ int annb_cellset_last_ms(annb_cellset_t *cs, float *probe_ms, float *walk_ms, fl
   if (walk_ms) *walk_ms = cs->walk_ms;
   if (merge_ms) *merge_ms = cs->merge_ms;
   if (route) *route = cs->last_route;
+  return ANNB_OK;
+}
+
+int annb_cellset_set_bruteforce(annb_cellset_t *cs, const int64_t *below) {
+  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  if (below)
+    for (int c = 0; c < cs->n_cells; c++)
+      if (below[c] < -1) ANNB_FAIL(ANNB_EINVAL, "cell %d: threshold %lld below -1", c, (long long)below[c]);
+  cs->below.assign((size_t)cs->n_cells, -1);
+  if (below) cs->below.assign(below, below + cs->n_cells);
+  return ANNB_OK;
+}
+
+int annb_cellset_last_scanned(annb_cellset_t *cs, int64_t *pairs, int64_t *rows) {
+  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  if (pairs) *pairs = cs->last_scanned_pairs;
+  if (rows) *rows = cs->last_scanned_rows;
   return ANNB_OK;
 }
 

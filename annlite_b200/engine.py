@@ -518,13 +518,23 @@ class CellSet:
             pass
 
     def search(self, queries, limit=10, ef=50, normalize=0, order=None, n_probe=None, generic=False, with_parts=False,
-               filter_ids=None, query_filter_ids=None):
+               filter_ids=None, query_filter_ids=None, bruteforce_below=None):
         """-> (labels uint64 (B, limit), dists fp32 (B, limit), cells int32 (B, limit)) [+ (part labels, part dists,
         part counters) (B, n_cells, limit / 3)].  `order` = (B, n_probe) cells per query, or None for the centroids'.
         `filter_ids` = one prepared filter id per cell (of that cell's Engine; 0 = the cell admits nothing), or None
         for no filter (annb_cellset_search_prepared / annb_cellset_search).  `query_filter_ids` = (B, n_cells): a
         prepared filter id of cell c's Engine for query q (0 = no filter for that query there), one filter per query
-        (annb_cellset_search_multi); exclusive with `filter_ids`."""
+        (annb_cellset_search_multi); exclusive with `filter_ids`.  `bruteforce_below` = (n_cells,) thresholds for the
+        filtered forms (HnswIndex.bruteforce_filter_below per cell, -1 = none), None = none: a cell's filter (or a
+        query's filter in a cell) that admits at most that many rows is scanned exactly instead of walked
+        (annb_cellset_set_bruteforce)."""
+        below = None
+        if bruteforce_below is not None:
+            below = np.ascontiguousarray(bruteforce_below, dtype=np.int64).reshape(-1)
+            if below.shape != (self.n_cells,):
+                raise ValueError(f'{below.shape[0]} bruteforce thresholds for {self.n_cells} cells')
+            if np.any(below < -1):
+                raise ValueError('bruteforce thresholds must be >= -1 (-1 = none)')
         q = Engine._as_f32(queries)
         B = q.shape[0]
         if order is not None:
@@ -549,6 +559,7 @@ class CellSet:
                 *([p.ctypes.data for p in parts] if parts else [None, None, None]))
         if filter_ids is not None and query_filter_ids is not None:
             raise ValueError('pass filter_ids or query_filter_ids, not both')
+        L.check(self._lib.annb_cellset_set_bruteforce(self._h, below.ctypes.data if below is not None else None))
         if query_filter_ids is not None:
             qids = np.ascontiguousarray(query_filter_ids, dtype=np.int32)
             if qids.shape != (B, self.n_cells):
@@ -565,10 +576,12 @@ class CellSet:
 
     def last_filtered(self):
         """What the last filtered search did besides the fused launch: (query, cell) pairs re-run on the bitmap walk,
-        and cells served by their own filtered launch."""
+        cells served by their own filtered launch, and (query, cell) pairs scanned exactly with the rows they scored."""
         a, b = C.c_int64(), C.c_int()
         L.check(self._lib.annb_cellset_last_filtered(self._h, C.byref(a), C.byref(b)))
-        return dict(rerun_pairs=a.value, handle_cells=b.value)
+        sp, sr = C.c_int64(), C.c_int64()
+        L.check(self._lib.annb_cellset_last_scanned(self._h, C.byref(sp), C.byref(sr)))
+        return dict(rerun_pairs=a.value, handle_cells=b.value, scanned_pairs=sp.value, scanned_rows=sr.value)
 
     def merge(self, labels, dists, counts, order, limit):
         """The merge alone over a by-cell scratch (host): labels / dists (B, n_cells, limit), counts (B, n_cells),

@@ -434,6 +434,22 @@ ANNB_API int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries,
 /* What the last annb_cellset_search_prepared / annb_cellset_search_multi did besides the fused launch: (query, cell)
  * pairs re-run on the bitmap walk, and cells served by their own filtered launch. */
 ANNB_API int annb_cellset_last_filtered(annb_cellset_t *cs, int64_t *rerun_pairs, int *handle_cells);
+/* Exact subset scans in the filtered cell-set searches (HnswIndex's bruteforce_filter_below per cell): below (host,
+ * n_cells entries, each >= -1; nullptr = all -1) = per cell, the largest filter count that is scanned instead of walked,
+ * -1 = never (the default: the searches launch and return exactly what they do without it).  In
+ * annb_cellset_search_prepared a cell whose filter has 0 < count <= below[c], and in annb_cellset_search_multi a pair
+ * (query, cell) with a filter and count <= below[c], is not walked: every probing query gets the k best of an exact ADC
+ * scan over the filter's rows -- a program's admitted rows in internal-id order, or a label list's entries that name
+ * live rows, in the list's order with repeats kept -- with the same k as the walk, sorted by (distance, position in
+ * that subset): annb_scan_subset's ids, distance bits and order.  The batch's K1 tables are built once, every subset
+ * is gathered once on the device, and one launch scans every pair (ANNB_CELLS_GENERIC and the per-cell route: one
+ * launch per cell).  A scanned pair with fewer live subset entries than its k gives ANNB_EFEWRESULTS.  The scan
+ * needs M = 8 one-byte codes with Ks = 256 (else ANNB_ELIMIT).  A scanned pair's part counters are {0 hops,
+ * 0 neighbours listed, rows scored}. */
+ANNB_API int annb_cellset_set_bruteforce(annb_cellset_t *cs, const int64_t *below);
+/* The (query, cell) pairs the last annb_cellset_search_prepared / annb_cellset_search_multi scanned exactly, and the
+ * rows those scans scored (the sum over scanned pairs of their subset's size). */
+ANNB_API int annb_cellset_last_scanned(annb_cellset_t *cs, int64_t *pairs, int64_t *rows);
 ANNB_API int annb_cellset_merge(annb_cellset_t *cs, const uint64_t *labels, const float *dists, const int32_t *counts,
                        const int32_t *order, int in_space, int64_t B, int n_probe, int limit, uint64_t *labels_out,
                        float *dists_out, int32_t *cells_out, int out_space);
