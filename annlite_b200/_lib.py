@@ -91,6 +91,8 @@ PROTOTYPES = {
                                          _vp, _vp, _vp]),
     'annb_cellset_last_filtered': (_int, [_vp, C.POINTER(_i64), C.POINTER(_int)]),
     'annb_cellset_set_bruteforce': (_int, [_vp, _vp]),
+    'annb_cellset_add_items': (_int, [_vp, _vp, _vp, _vp, _i64, _int]),
+    'annb_cellset_last_build': (_int, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(_i64), C.POINTER(_int)]),
     'annb_cellset_last_scanned': (_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
     'annb_cellset_merge': (_int, [_vp, _vp, _vp, _vp, _vp, _int, _i64, _int, _int, _vp, _vp, _vp, _int]),
     'annb_cellset_probe': (_int, [_vp, _vp, _int, _i64, _int, _vp, _int]),

@@ -123,21 +123,45 @@ class CellContainer:
                 self._vec_indexes[old].delete([label])
                 self._live[old] -= 1
                 del self._label_cell[label]
-        for c in np.unique(cells).tolist():
-            sel = np.flatnonzero(cells == c)
-            idx = self._vec_indexes[c]
-            attrs = None
+        targets = np.unique(cells).tolist()
+        shares = {c: np.flatnonzero(cells == c) for c in targets}
+        attrs = {}
+        for c in targets:
+            sel, idx = shares[c], self._vec_indexes[c]
             if tags is not None and idx.attributes.names:
                 rows = [tags[i] for i in sel] if not isinstance(tags, dict) else {k: [v[i] for i in sel] for k, v in tags.items()}
-                attrs = idx.attributes.convert(rows, len(sel))
-            # (the default call is the plain add_with_ids(x, ids): any cell index with that interface works)
-            idx.add_with_ids(data[sel], ids[sel], **({} if num_threads == -1 else {'num_threads': num_threads}))
-            if attrs is not None:
-                idx.set_attributes(ids[sel], attrs)
+                attrs[c] = idx.attributes.convert(rows, len(sel))
+        if self._one_call(targets, num_threads):
+            # every cell's share in one cell-set insertion: each graph comes out as its own add_with_ids makes it, and
+            # the shares that build on the GPU are built together
+            x = np.empty((n, self.n_dim), dtype=np.float32)
+            for c in targets:
+                x[shares[c]] = self._vec_indexes[c]._rows_to_add(data[shares[c]], ids[shares[c]])
+            self._cells().add_items(x, ids.astype(np.uint64), cells, num_threads=self._threads(targets[0], num_threads))
+            for c in targets:
+                self._vec_indexes[c]._index.added(len(shares[c]))
+        else:
+            for c in targets:
+                # (the default call is the plain add_with_ids(x, ids): any cell index with that interface works)
+                self._vec_indexes[c].add_with_ids(data[shares[c]], ids[shares[c]],
+                                                  **({} if num_threads == -1 else {'num_threads': num_threads}))
+        for c in targets:
+            sel = shares[c]
+            if c in attrs:
+                self._vec_indexes[c].set_attributes(ids[sel], attrs[c])
             for label in ids[sel].tolist():
                 if label not in self._label_cell:
                     self._live[c] += 1
                 self._label_cell[label] = c
+
+    def _threads(self, c, num_threads):
+        return self._vec_indexes[c]._index.threads_for(num_threads)
+
+    def _one_call(self, targets, num_threads):
+        """The batch can be one cell-set insertion: GPU HnswIndex cells that would all insert with one thread count."""
+        if not all(isinstance(v, HnswIndex) and v.device >= 0 for v in self._vec_indexes):
+            return False
+        return len({self._threads(c, num_threads) for c in targets}) == 1
 
     def update(self, data: 'np.ndarray', cells: 'np.ndarray', ids, tags=None, num_threads: int = -1):
         self.insert(data, cells, ids=ids, tags=tags, num_threads=num_threads)

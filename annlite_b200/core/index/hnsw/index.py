@@ -258,16 +258,23 @@ class HnswIndex:
     # ---- BaseIndex surface ------------------------------------------------------------------------
     def add_with_ids(self, x: 'np.ndarray', ids: List[int], num_threads: int = -1):
         """hnsw/index.py:125-137.  Codes and per-row tables come from the device in chunks."""
+        x = self._rows_to_add(x, ids)
+        self._index.add_vectors(x, ids=np.asarray(ids, dtype=np.uint64), num_threads=num_threads)
+
+    def _rows_to_add(self, x, ids):
+        """add_with_ids' steps before the insertion itself: capacity grown for the largest id, rows as fp32, and for
+        COSINE pre_process's normalisation (the library adds get_dist_mat's own pass).  CellContainer.insert calls it
+        for each cell before inserting every cell's rows in one call."""
         self._ensure_backend()
         x = self._prep(x)
         max_id = int(max(ids)) + 1
         if max_id > self.capacity:
             expand_steps = math.ceil(max_id / self.expand_step_size)
             self._expand_capacity(expand_steps * self.expand_step_size)
-        if self.metric == Metric.COSINE:   # pre_process's pass; the library adds get_dist_mat's own pass
+        if self.metric == Metric.COSINE:
             from ....math import l2_normalize
             x = np.ascontiguousarray(l2_normalize(x), dtype=np.float32)
-        self._index.add_vectors(x, ids=np.asarray(ids, dtype=np.uint64), num_threads=num_threads)
+        return x
 
     def search(self, query: 'np.ndarray', limit: int = 10, indices: Optional['np.ndarray'] = None):
         """hnsw/index.py:140-167: one query -> (dists[limit], ids[limit]); EUCLIDEAN gets sqrt."""

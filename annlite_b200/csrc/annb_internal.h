@@ -423,4 +423,25 @@ int hnsw_host_add(annb_index *h, const float *vectors, const void *codes, const 
                   const int32_t *forced_levels);
 // level-0 insertion on the GPU (gpu_build.cu); 1 = not applicable, take the host path
 int gpu_build_run(annb_index *h, const float *vectors, const uint64_t *labels, int64_t n, int num_threads);
+// ... the handle-side part of its rule (geometry, codebook copy, no deletions)
+bool gpu_build_geometry(const annb_index *h);
+// One cell's share of a cell-set insertion that gpu_build_run would build on the GPU (annb_cellset_add_items)
+struct CellBuildJob {
+  annb_index *h = nullptr;
+  int cell = 0;                   // its index in the cell set (error messages)
+  const float *vectors = nullptr; // every row of the call (n, dim)
+  std::vector<int64_t> rows;      // the cell's rows of the call, in order
+  std::vector<uint64_t> labels;   // their labels
+};
+struct CellBuildStats {
+  double phase1_ms = 0, phase2_ms = 0;
+  int64_t rounds = 0;
+};
+// gpu_build_run for every job at once: phase 1 on a host thread per cell, phase 2 in rounds of every cell's next batch
+// on drv's stream (M = 8 codes shared by all cells); each graph comes out as gpu_build_run makes it alone
+int gpu_build_cells(annb_index *drv, std::vector<CellBuildJob> &jobs, int num_threads, CellBuildStats *stats);
+// capi.cu: what annb_add_items(h, vectors, NULL, labels, n, num_threads) refuses up front (*gpu = it takes the GPU
+// builder), and its steps before inserting; the caller holds the handle lock
+int add_items_check(annb_index *h, const uint64_t *labels, int64_t n, int num_threads, bool *gpu);
+int add_items_enter(annb_index *h);
 int sync_device_graph(annb_index *h);

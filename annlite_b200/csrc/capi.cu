@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <unordered_set>
 
 #include "annb_internal.h"
 
@@ -707,6 +708,34 @@ int hnsw_host_add(annb_index *h, const float *vectors, const void *codes, const 
   }
   if (rc == ANNB_ECUDA && f.rc) return f.rc;
   return rc;
+}
+
+// What annb_add_items(h, vectors, NULL, labels, n, num_threads) would refuse before it inserts anything (the handle lock
+// held); *gpu = it would take the GPU builder (gpu_build_run applies: >= 16384 fresh rows, no stored or repeated labels).
+int add_items_check(annb_index *h, const uint64_t *labels, int64_t n, int num_threads, bool *gpu) {
+  *gpu = false;
+  if (h->device < 0) ANNB_FAIL(ANNB_ENODEVICE, "this handle is host-only (graph I/O); compute needs a CUDA device: annlite_b200 has no CPU fallback");
+  if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
+  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised: call annb_init_graph first");
+  const HostGraph &g = h->g;
+  const bool try_gpu = num_threads != 1 && h->opt_gpu_build && n >= 16384 && gpu_build_geometry(h);
+  if (try_gpu && g.count.load() + n > g.max_elements) ANNB_FAIL(ANNB_ECAPACITY, "The number of elements exceeds the specified limit");
+  int64_t fresh = 0;
+  std::unordered_set<uint64_t> seen;
+  for (int64_t i = 0; i < n; i++)
+    if (g.label_lookup.find(labels[i]) == g.label_lookup.end() && seen.insert(labels[i]).second) fresh++;
+  if (g.count.load() + fresh > g.max_elements) ANNB_FAIL(ANNB_ECAPACITY, "The number of elements exceeds the specified limit");
+  *gpu = try_gpu && fresh == n;
+  return ANNB_OK;
+}
+
+// annb_add_items' steps before an insertion (the handle lock held): streamed work settled, the state moved on
+int add_items_enter(annb_index *h) {
+  ANNB_TRY(settle_flagged_lanes(h));
+  h->state_gen++;
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream2));
+  return ANNB_OK;
 }
 
 

@@ -31,6 +31,8 @@ struct annb_cellset {
   std::vector<int64_t> below;       // annb_cellset_set_bruteforce: per cell, scan filters admitting <= this many (-1 = never)
   int64_t last_scanned_pairs = 0;   // (query, cell) pairs the last filtered search scanned exactly ...
   int64_t last_scanned_rows = 0;    // ... and the rows those scans scored
+  CellBuildStats build;             // annb_cellset_add_items: the last call's one-pass build ...
+  int build_cells = 0;              // ... and the cells it served
 };
 
 namespace {
@@ -1308,6 +1310,95 @@ int annb_cellset_last_filtered(annb_cellset_t *cs, int64_t *rerun_pairs, int *ha
   if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
   if (rerun_pairs) *rerun_pairs = cs->last_rerun_pairs;
   if (handle_cells) *handle_cells = cs->last_handle_cells;
+  return ANNB_OK;
+}
+
+// Rows split by cell, each cell's share in input order.  A share that annb_add_items would build on the GPU (>= 16384
+// fresh rows, no deletions, gpu_build_run's geometry) goes through gpu_build_cells together with the other such shares:
+// phase 1 on a host thread per cell, phase 2 in rounds with one multi-cell walk and two link launches for all of them.
+// Every other share is annb_add_items on its own handle.  Each cell's graph is what its own annb_add_items makes.
+int annb_cellset_add_items(annb_cellset_t *cs, const float *vectors, const uint64_t *labels, const int32_t *cells, int64_t n,
+                           int num_threads) {
+  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  if (n < 0 || (n > 0 && (!vectors || !labels || !cells))) ANNB_FAIL(ANNB_EINVAL, "null vectors/labels/cells");
+  const int C = cs->n_cells;
+  std::vector<std::vector<int64_t>> rows((size_t)C);
+  for (int64_t i = 0; i < n; i++) {
+    const int32_t c = cells[i];
+    if (c < 0 || c >= C) ANNB_FAIL(ANNB_EINVAL, "row %lld: %d is not a cell of the set (n_cells=%d)", (long long)i, c, C);
+    rows[(size_t)c].push_back(i);
+  }
+  cs->build = CellBuildStats();
+  cs->build_cells = 0;
+  if (n == 0) return ANNB_OK;
+  ANNB_CUDA(cudaSetDevice(cs->device));
+  // every share is checked before anything is inserted
+  std::vector<std::vector<uint64_t>> lab((size_t)C);
+  std::vector<char> one_pass((size_t)C, 0);
+  for (int c = 0; c < C; c++) {
+    if (rows[c].empty()) continue;
+    lab[c].resize(rows[c].size());
+    for (size_t t = 0; t < rows[c].size(); t++) lab[c][t] = labels[rows[c][t]];
+    annb_index *h = cs->cells[c];
+    bool gpu;
+    int rc;
+    {
+      std::lock_guard<std::mutex> lk(h->mu);
+      rc = add_items_check(h, lab[c].data(), (int64_t)lab[c].size(), num_threads, &gpu);
+    }
+    if (rc) {
+      const std::string msg = annb_last_error();
+      ANNB_FAIL(rc, "cell %d: %s", c, msg.c_str());
+    }
+    // the multi-cell walk has the M = 8 geometry; one walk launch has one table form
+    one_pass[c] = gpu && h->M == 8 && h->opt_ip_raw == cs->h0->opt_ip_raw;
+  }
+  std::vector<float> v;
+  for (int c = 0; c < C; c++) {
+    if (rows[c].empty() || one_pass[c]) continue;
+    v.resize(rows[c].size() * (size_t)cs->dim);
+    for (size_t t = 0; t < rows[c].size(); t++)
+      memcpy(v.data() + t * cs->dim, vectors + (size_t)rows[c][t] * cs->dim, (size_t)cs->dim * 4);
+    const int rc = annb_add_items(cs->cells[c], v.data(), nullptr, lab[c].data(), (int64_t)lab[c].size(), num_threads);
+    if (rc) {
+      const std::string msg = annb_last_error();
+      ANNB_FAIL(rc, "cell %d: %s", c, msg.c_str());
+    }
+  }
+  std::vector<CellBuildJob> jobs;
+  for (int c = 0; c < C; c++) {
+    if (!one_pass[c]) continue;
+    jobs.emplace_back();
+    CellBuildJob &j = jobs.back();
+    j.h = cs->cells[c];
+    j.cell = c;
+    j.vectors = vectors;
+    j.rows = std::move(rows[c]);
+    j.labels = std::move(lab[c]);
+  }
+  if (jobs.empty()) return ANNB_OK;
+  // cell 0's stream and scratch run phase 2: its lock is taken too (cells in ascending order)
+  std::vector<std::unique_lock<std::mutex>> locks;
+  if (!one_pass[0]) locks.emplace_back(cs->h0->mu);
+  for (CellBuildJob &j : jobs) {
+    locks.emplace_back(j.h->mu);
+    const int rc = add_items_enter(j.h);
+    if (rc) {
+      const std::string msg = annb_last_error();
+      ANNB_FAIL(rc, "cell %d: %s", j.cell, msg.c_str());
+    }
+  }
+  ANNB_CUDA(cudaStreamSynchronize(cs->h0->stream));
+  cs->build_cells = (int)jobs.size();
+  return gpu_build_cells(cs->h0, jobs, num_threads, &cs->build);
+}
+
+int annb_cellset_last_build(annb_cellset_t *cs, double *phase1_ms, double *phase2_ms, int64_t *rounds, int *cells) {
+  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  if (phase1_ms) *phase1_ms = cs->build.phase1_ms;
+  if (phase2_ms) *phase2_ms = cs->build.phase2_ms;
+  if (rounds) *rounds = cs->build.rounds;
+  if (cells) *cells = cs->build_cells;
   return ANNB_OK;
 }
 

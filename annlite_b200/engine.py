@@ -574,6 +574,26 @@ class CellSet:
             L.check(self._lib.annb_cellset_search_prepared(*head, fids.ctypes.data, *tail))
         return (labels, dists, cells) + ((parts,) if with_parts else ())
 
+    def add_items(self, vectors, labels, cells, num_threads=-1):
+        """Insert host rows (n, dim) with their labels into the given cells (n,) (annb_cellset_add_items): each cell's
+        graph is what its Engine.add_items of its rows, in order, makes; the shares that build on the GPU are built
+        together, the others one cell at a time."""
+        v = np.ascontiguousarray(vectors, dtype=np.float32)
+        lab = np.ascontiguousarray(labels, dtype=np.uint64).reshape(-1)
+        cel = np.ascontiguousarray(cells, dtype=np.int32).reshape(-1)
+        if v.ndim != 2 or v.shape[1] != self.engines[0].dim:
+            raise ValueError(f'rows of shape {v.shape} for cells of dim {self.engines[0].dim}')
+        if lab.shape[0] != v.shape[0] or cel.shape[0] != v.shape[0]:
+            raise ValueError(f'{lab.shape[0]} labels and {cel.shape[0]} cells for {v.shape[0]} rows')
+        L.check(self._lib.annb_cellset_add_items(self._h, v.ctypes.data, lab.ctypes.data, cel.ctypes.data, v.shape[0],
+                                                 int(num_threads)))
+
+    def last_build(self):
+        """The last add_items' one-pass build: phase-1 and phase-2 host ms, rounds, and the cells it built."""
+        a, b, r, c = C.c_double(), C.c_double(), C.c_int64(), C.c_int()
+        L.check(self._lib.annb_cellset_last_build(self._h, C.byref(a), C.byref(b), C.byref(r), C.byref(c)))
+        return dict(phase1_ms=a.value, phase2_ms=b.value, rounds=r.value, cells=c.value)
+
     def last_filtered(self):
         """What the last filtered search did besides the fused launch: (query, cell) pairs re-run on the bitmap walk,
         cells served by their own filtered launch, and (query, cell) pairs scanned exactly with the rows they scored."""

@@ -171,9 +171,16 @@ class Index:
         self._need_pq()
         v = np.ascontiguousarray(vectors, dtype=np.float32)
         labels = self._labels_for(ids, v.shape[0])
-        nt = self.num_threads if num_threads <= 0 else int(num_threads)
-        self._e.add_items(v, labels, codes=codes, num_threads=nt)
-        self._cur_l += v.shape[0]
+        self._e.add_items(v, labels, codes=codes, num_threads=self.threads_for(num_threads))
+        self.added(v.shape[0])
+
+    def threads_for(self, num_threads):
+        """The thread count an insertion with this num_threads argument uses (<= 0: the index's own)."""
+        return self.num_threads if num_threads <= 0 else int(num_threads)
+
+    def added(self, rows):
+        """Bookkeeping after `rows` rows went into the engine (by add_vectors or a cell-set insertion)."""
+        self._cur_l += rows
         self.ep_added = True
 
     # ---- search ---------------------------------------------------------------------------

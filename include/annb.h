@@ -459,6 +459,21 @@ ANNB_API int annb_cellset_probe(annb_cellset_t *cs, const float *queries, int in
 /* Device time of the last probe / walk (fused launch, or the per-cell searches) / merge in ms, and the route the last
  * annb_cellset_search* call took (0 = fused walk, 1 = per-cell searches; annb_cellset_search_multi: own launches). */
 ANNB_API int annb_cellset_last_ms(annb_cellset_t *cs, float *probe_ms, float *walk_ms, float *merge_ms, int *route);
+/* Insertion into a cell set: host fp32 rows (n, dim), their labels and a target cell per row (int32).  Rows are split
+ * by cell, each cell keeping its rows in input order, and every cell's graph comes out exactly as
+ * annb_add_items(cell, its rows, NULL, its labels, its row count, num_threads) makes it (save_index bytes, labels,
+ * levels, codes).  The shares annb_add_items would build on the GPU -- at least 16384 fresh rows, no deletions, no
+ * stored or repeated labels, num_threads != 1, Ks = 256 one-byte codes, and here M = 8 -- are built together: phase 1
+ * on a host thread per cell, then phase 2 in rounds where every such cell inserts its next batch (the size its own build
+ * would pick), with one multi-cell walk launch per round (more when a round's by-cell scratch would pass 256 MB or the
+ * cells' ef_construction differ), one encode launch per cell, and two link launches.  Every other share is
+ * annb_add_items on its own handle.  Every share is checked first: an error names the cell, and a share that would
+ * overrun its cell's capacity gives ANNB_ECAPACITY before anything is inserted. */
+ANNB_API int annb_cellset_add_items(annb_cellset_t *cs, const float *vectors, const uint64_t *labels, const int32_t *cells,
+                           int64_t n, int num_threads);
+/* The last annb_cellset_add_items' one-pass build: host time of phase 1 and of phase 2 with the host graphs'
+ * assembly in ms, its rounds, and the cells it built (0 = every share went through annb_add_items). */
+ANNB_API int annb_cellset_last_build(annb_cellset_t *cs, double *phase1_ms, double *phase2_ms, int64_t *rounds, int *cells);
 
 /* ---- introspection for bench / roofline ------------------------------------------------------ */
 /* Device time of the last search / scan / table kernel in milliseconds (CUDA events on the
