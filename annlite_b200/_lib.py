@@ -103,6 +103,7 @@ PROTOTYPES = {
     'annb_fallback_count': (_int, [_vp, C.POINTER(_i64)]),
     'annb_fallback_queries': (_int, [_vp, C.POINTER(_i64)]),
     'annb_sync_counts': (_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
+    'annb_device_graph_layout': (_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_int)]),
     'annb_set_option': (_int, [_vp, _cp, _i64]),
 }
 

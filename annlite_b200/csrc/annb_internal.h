@@ -114,6 +114,20 @@ struct GraphDev {
   alignas(16) uint8_t ep_code[128];     // code of the entry node (code_row <= 128 bytes)
 };
 
+// Wide code rows (ANNB_NARROW_CODE_ROW < code_row <= ANNB_MAX_CODE_ROW): co-locating maxM0 neighbour codes would make a
+// level-0 record maxM0 x code_row bytes (24.6 KB at M = 768), so the GraphDev records hold links only and every node's
+// code is stored once in a by-internal-id matrix.  GraphDev then reads:
+//   level-0 record r0[id]  : [maxM0 x u32 link = node id][pad to 16]                          (rec0_bytes, code_off0 = 0)
+//   upper record  up[l][r] : [maxM x u32 link = record index at level l][pad to 16][maxM x u32 node id of that link]
+//                            [pad to 8][u32 node id][u32 down][pad to 16]       (recu_bytes; node ids at code_offu)
+// and ep_code is unused.  What hnsw_walk_wide reads besides GraphDev and SearchParams:
+struct WideDev {
+  const uint8_t *codes;   // n x code_stride, node id -> code row (16-byte aligned rows)
+  const float *codebook;  // (M, Ks, ds) fp32, as annb_set_codebook received it
+  int64_t code_stride;    // bytes between two code rows
+  int32_t dim;
+};
+
 struct SearchParams {
   const float *tables;  // (B, M, Ks), or nullptr when the walk builds its tables itself (fused K1, hnsw_walk4)
   const float *queries; // (B, D) device, already normalised where the metric asks for it; nullptr = use `tables`
@@ -271,6 +285,9 @@ struct annb_index {
   uint8_t *d_own_codes = nullptr;
   size_t cap_own_codes = 0;
   uint64_t own_codes_gen = 0;
+  // wide code rows: the by-id code matrix the walk reads (WideDev::codes), kept with the device graph
+  uint8_t *d_wide_codes = nullptr;
+  size_t cap_wide_codes = 0;
 
   // scratch (grown on demand)
   void *d_scratch[40] = {nullptr};
@@ -361,6 +378,12 @@ int launch_scatter_records(annb_index *h, const uint8_t *d_staged, const uint32_
 // mode: 0 = fast walk (no filter, no deletions), 1 = filtered/deleted walk, kernel chosen automatically
 // (flagged single-list walk when its list fits, else the bitmap walk), 2 = bitmap walk
 int launch_search(annb_index *h, const SearchParams &p, int mode);
+// code rows wider than ANNB_NARROW_CODE_ROW: links-only device records, the by-id code matrix and hnsw_walk_wide
+inline bool wide_rows(const annb_index *h) { return (size_t)h->M * h->code_bytes > ANNB_NARROW_CODE_ROW; }
+inline int64_t wide_code_stride(const annb_index *h) { return ((int64_t)h->M * h->code_bytes + 15) / 16 * 16; }
+// hnsw_walk_wide (walk_wide.cu): every search mode of launch_search for a wide index; distances from p.queries and the
+// codebook (p.tables == nullptr) or from p.tables
+int launch_walk_wide(annb_index *h, const SearchParams &p);
 // hnsw_walk4 (walk_fused.cu): the plain search with the table built inside the walk; returns 1 = not applicable
 bool walk4_applicable(const annb_index *h);
 bool walk4_can_fuse(const annb_index *h);

@@ -8,7 +8,7 @@ NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
 ARCH="-gencode arch=compute_90a,code=sm_90a"
 CXXFLAGS="-O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function ${ANNB_EXTRA_NVCC:-}"
 pids=()
-for f in adc_table adc_scan hnsw_search walk_fused walk_flagged4 gpu_build attr_filter cells capi; do
+for f in adc_table adc_scan hnsw_search walk_fused walk_flagged4 walk_wide gpu_build attr_filter cells capi; do
   $NVCC $ARCH $CXXFLAGS -c "$HERE/$f.cu" -o "$HERE/obj/$f.o" &
   pids+=($!)
 done
@@ -17,6 +17,6 @@ g++ -O3 -std=c++17 -fPIC -fvisibility=hidden -ffp-contract=off -march=x86-64-v3 
     -c "$HERE/hnsw_build.cpp" -o "$HERE/obj/hnsw_build.o" &
 pids+=($!)
 for p in "${pids[@]}"; do wait "$p"; done
-$NVCC $ARCH -shared -o "$OUT/libannlite_b200.so" "$HERE"/obj/{adc_table,adc_scan,hnsw_search,walk_fused,walk_flagged4,gpu_build,attr_filter,cells,capi,hnsw_build}.o \
+$NVCC $ARCH -shared -o "$OUT/libannlite_b200.so" "$HERE"/obj/{adc_table,adc_scan,hnsw_search,walk_fused,walk_flagged4,walk_wide,gpu_build,attr_filter,cells,capi,hnsw_build}.o \
     -Xlinker --exclude-libs,ALL -lpthread
 echo "built $OUT/libannlite_b200.so"

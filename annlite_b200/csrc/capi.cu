@@ -152,9 +152,10 @@ int annb_create(int device, int metric, int dim, int n_subvectors, int n_cluster
   h->Ks = n_clusters;
   h->ds = dim / n_subvectors;
   h->code_bytes = n_clusters <= 256 ? 1 : 2;
-  if ((size_t)h->M * h->code_bytes > 128) {
+  if ((size_t)h->M * h->code_bytes > ANNB_MAX_CODE_ROW) {
     delete h;
-    ANNB_FAIL(ANNB_ELIMIT, "code rows wider than 128 bytes are not supported (n_subvectors=%d)", n_subvectors);
+    ANNB_FAIL(ANNB_ELIMIT, "code rows wider than ANNB_MAX_CODE_ROW=%d bytes are not supported (n_subvectors=%d x %d-byte codes)",
+              ANNB_MAX_CODE_ROW, n_subvectors, n_clusters <= 256 ? 1 : 2);
   }
   if (device < 0) {
     *out = h;
@@ -193,6 +194,7 @@ int annb_destroy(annb_index_t *h) {
   if (h->d_labels) cudaFree(h->d_labels);
   if (h->d_deleted) cudaFree(h->d_deleted);
   if (h->d_own_codes) cudaFree(h->d_own_codes);
+  if (h->d_wide_codes) cudaFree(h->d_wide_codes);
   for (AttrColumn &c : h->attrs) {
     if (c.d_vals) cudaFree(c.d_vals);
     if (c.d_valid) cudaFree(c.d_valid);
@@ -302,6 +304,14 @@ static int build_tables(annb_index *h, const float *queries, int q_space, int64_
   return ANNB_OK;
 }
 
+// Queries whose K1 tables an exhaustive scan builds at once: all B for code rows of <= 128 bytes; for wider rows a
+// table is M x Ks x 4 bytes (786 KB at M = 768), so the batch is scanned a chunk at a time within a fixed scratch cap.
+static int64_t table_chunk_rows(const annb_index *h, int64_t B) {
+  if (!wide_rows(h)) return std::max<int64_t>(B, 1);
+  const size_t cap = (size_t)256 << 20, per = (size_t)h->M * h->Ks * sizeof(float);
+  return std::max<int64_t>(1, std::min<int64_t>(B, (int64_t)(cap / per)));
+}
+
 // fill the fused-build fields of a SearchParams (hnsw_walk4 builds each query's table in shared memory)
 static void fuse_params(annb_index *h, SearchParams &p, const float *d_queries) {
   p.tables = nullptr;
@@ -399,25 +409,30 @@ int annb_scan_topk(annb_index_t *h, const float *queries, const float *tables, i
   if (B < 0 || k <= 0 || !ids || !dists) ANNB_FAIL(ANNB_EINVAL, "bad B/k/outputs");
   if (!h->d_codes) ANNB_FAIL(ANNB_ESTATE, "no code matrix: call annb_set_codes first");
   if (B == 0) return ANNB_OK;
-  const size_t tbytes = (size_t)B * h->M * h->Ks * sizeof(float);
-  const float *dt;
-  if (tables) {
-    ANNB_TRY(stage_in(h, tables, in_space, tbytes, S_TABLES, (const void **)&dt));
-  } else {
-    float *t;
-    ANNB_TRY(annb_scratch(h, S_TABLES, tbytes, (void **)&t));
-    // PQIndex.search builds its table with precompute_adc (L2 form, no normalisation): pq.py:200-224
-    ANNB_TRY(build_tables(h, queries, in_space, B, 0, t));
-    dt = t;
-  }
+  const size_t TS = (size_t)h->M * h->Ks;
   int64_t *dids = ids;
   float *dd = dists;
   if (out_space != ANNB_DEVICE) {
     ANNB_TRY(annb_scratch(h, S_OUT_L, (size_t)B * k * sizeof(int64_t), (void **)&dids));
     ANNB_TRY(annb_scratch(h, S_OUT_D, (size_t)B * k * sizeof(float), (void **)&dd));
   }
-  if (h->opt_timing) cudaEventRecord(h->ev[4], h->stream);
-  ANNB_TRY(launch_scan_topk(h, dt, B, k, dids, dd));
+  const int64_t step = table_chunk_rows(h, B);
+  for (int64_t b0 = 0; b0 < B; b0 += step) {
+    const int64_t nb = std::min(step, B - b0);
+    const size_t tbytes = (size_t)nb * TS * sizeof(float);
+    const float *dt;
+    if (tables) {
+      ANNB_TRY(stage_in(h, tables + (size_t)b0 * TS, in_space, tbytes, S_TABLES, (const void **)&dt));
+    } else {
+      float *t;
+      ANNB_TRY(annb_scratch(h, S_TABLES, tbytes, (void **)&t));
+      // PQIndex.search builds its table with precompute_adc (L2 form, no normalisation): pq.py:200-224
+      ANNB_TRY(build_tables(h, queries + (size_t)b0 * h->dim, in_space, nb, 0, t));
+      dt = t;
+    }
+    if (h->opt_timing && b0 == 0) cudaEventRecord(h->ev[4], h->stream);
+    ANNB_TRY(launch_scan_topk(h, dt, nb, k, dids + b0 * k, dd + b0 * k));
+  }
   if (h->opt_timing) cudaEventRecord(h->ev[5], h->stream);
   if (out_space != ANNB_DEVICE) {
     ANNB_CUDA(cudaMemcpyAsync(ids, dids, (size_t)B * k * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
@@ -686,7 +701,9 @@ int hnsw_host_add(annb_index *h, const float *vectors, const void *codes, const 
   f.vectors = vectors;
   f.n = n;
   const size_t TS = (size_t)h->M * h->Ks;
-  f.chunk_rows = std::max<int64_t>(64, std::min<int64_t>(8192, (int64_t)((64u << 20) / (TS * sizeof(float)))));
+  // about 64 MB of tables per chunk; wide rows (up to 134 MB per row at M = 512, Ks = 65 536) go down to one row
+  const int64_t min_rows = wide_rows(h) ? 1 : 64;
+  f.chunk_rows = std::max<int64_t>(min_rows, std::min<int64_t>(8192, (int64_t)((64u << 20) / (TS * sizeof(float)))));
   f.rc = 0;
   for (int b = 0; b < 2; b++) {
     ANNB_TRY(annb_pinned(h, b, (size_t)f.chunk_rows * TS * sizeof(float), (void **)&f.pinned[b]));
@@ -866,6 +883,7 @@ static int upload_upper(annb_index *h) {
   d.maxlevel = g.maxlevel;
   d.ep_node = g.enterpoint;
   if (g.maxlevel >= ANNB_MAX_LEVELS) ANNB_FAIL(ANNB_ELIMIT, "graph has %d levels (limit %d)", g.maxlevel + 1, ANNB_MAX_LEVELS);
+  const bool wide = wide_rows(h);  // upper records carry the links' node ids instead of their codes
   std::vector<uint8_t> up;
   std::vector<uint32_t> map_prev, map_cur;
   size_t off = 0;
@@ -891,7 +909,8 @@ static int upload_upper(annb_index *h) {
           memcpy(&v, ll + 4 + 4 * j, 4);
           if (map_cur[v] == 0xffffffffu) ANNB_FAIL(ANNB_EINVAL, "Trying to make a link on a non-existent level");
           lk = map_cur[v];
-          memcpy(rec + d.code_offu + (size_t)j * d.code_row, g.code(v), (size_t)d.code_row);
+          if (wide) memcpy(rec + d.code_offu + (size_t)j * 4, &v, 4);
+          else memcpy(rec + d.code_offu + (size_t)j * d.code_row, g.code(v), (size_t)d.code_row);
         }
         links[j] = lk;
       }
@@ -906,7 +925,7 @@ static int upload_upper(annb_index *h) {
   ANNB_TRY(ensure_dev((void **)&h->d_up, &h->cap_up, std::max<size_t>(up.size(), 16)));
   if (!up.empty()) ANNB_CUDA(cudaMemcpyAsync(h->d_up, up.data(), up.size(), cudaMemcpyHostToDevice, h->stream));
   d.up = h->d_up;
-  memcpy(d.ep_code, g.code(g.enterpoint), (size_t)d.code_row);
+  if (!wide) memcpy(d.ep_code, g.code(g.enterpoint), (size_t)d.code_row);  // a wide walk reads it from the code matrix
   return ANNB_OK;
 }
 
@@ -921,7 +940,12 @@ static int patch_device_graph(annb_index *h) {
   std::sort(ids.begin(), ids.end());
   ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
   const size_t cnt = ids.size();
-  if (h->patch.untracked || n < n_old || cnt > (size_t)n / 4 + 64 || (size_t)n * d.rec0_bytes > h->cap_rec0 || (size_t)n * 8 > h->cap_labels) {
+  // wide code rows: records hold links only, and the new nodes' rows are appended to the by-id code matrix (the
+  // tracked insertion only adds nodes; an in-place update is untracked)
+  const bool wide = wide_rows(h);
+  const size_t stride = (size_t)wide_code_stride(h);
+  if (h->patch.untracked || n < n_old || cnt > (size_t)n / 4 + 64 || (size_t)n * d.rec0_bytes > h->cap_rec0 || (size_t)n * 8 > h->cap_labels ||
+      (wide && (size_t)n * stride > h->cap_wide_codes)) {
     h->dev_dirty = true;   // too much changed, or the device buffers are too small: re-derive everything
     return 1;
   }
@@ -942,10 +966,16 @@ static int patch_device_graph(annb_index *h) {
       uint32_t lk = 0xffffffffu;
       if (j < (int)c) {
         memcpy(&lk, ll + 4 + 4 * j, 4);
-        memcpy(rec + d.code_off0 + (size_t)j * d.code_row, g.code(lk), (size_t)d.code_row);
+        if (!wide) memcpy(rec + d.code_off0 + (size_t)j * d.code_row, g.code(lk), (size_t)d.code_row);
       }
       links[j] = lk;
     }
+  }
+  if (wide && n > n_old) {
+    std::vector<uint8_t> rows((size_t)(n - n_old) * stride, 0);
+    for (int64_t i = n_old; i < n; i++) memcpy(rows.data() + (size_t)(i - n_old) * stride, g.code((uint32_t)i), (size_t)d.code_row);
+    ANNB_CUDA(cudaMemcpyAsync(h->d_wide_codes + (size_t)n_old * stride, rows.data(), rows.size(), cudaMemcpyHostToDevice, h->stream));
+    ANNB_CUDA(cudaStreamSynchronize(h->stream));  // `rows` goes out of scope
   }
   uint8_t *dst;
   uint32_t *did;
@@ -998,10 +1028,18 @@ int sync_device_graph(annb_index *h) {
   d.maxM = g.maxM;
   d.maxM0 = g.maxM0;
   auto up16 = [](size_t v) { return (v + 15) / 16 * 16; };
-  d.code_off0 = (int)up16((size_t)4 * g.maxM0);
-  d.rec0_bytes = (int)up16((size_t)d.code_off0 + (size_t)g.maxM0 * d.code_row);
-  d.code_offu = (int)up16((size_t)4 * g.maxM);
-  d.tail_offu = (int)(((size_t)d.code_offu + (size_t)g.maxM * d.code_row + 7) / 8 * 8);
+  const bool wide = wide_rows(h);
+  if (wide) {  // links only; upper records carry their links' node ids (annb_internal.h: WideDev)
+    d.code_off0 = 0;
+    d.rec0_bytes = (int)up16((size_t)4 * g.maxM0);
+    d.code_offu = (int)up16((size_t)4 * g.maxM);
+    d.tail_offu = (int)(((size_t)d.code_offu + (size_t)g.maxM * 4 + 7) / 8 * 8);
+  } else {
+    d.code_off0 = (int)up16((size_t)4 * g.maxM0);
+    d.rec0_bytes = (int)up16((size_t)d.code_off0 + (size_t)g.maxM0 * d.code_row);
+    d.code_offu = (int)up16((size_t)4 * g.maxM);
+    d.tail_offu = (int)(((size_t)d.code_offu + (size_t)g.maxM * d.code_row + 7) / 8 * 8);
+  }
   d.recu_bytes = (int)up16((size_t)d.tail_offu + 8);
   d.maxlevel = g.maxlevel;
   d.ep_node = g.enterpoint;
@@ -1020,6 +1058,12 @@ int sync_device_graph(annb_index *h) {
   ANNB_TRY(ensure_dev((void **)&h->d_rec0, &h->cap_rec0, (size_t)n_alloc * d.rec0_bytes));
   d.rec0 = h->d_rec0;
   ANNB_TRY(launch_pack_rec0(h, raw, n));
+  if (wide) {  // every node's code row, once, from the reference-layout records already on the device
+    const size_t stride = (size_t)wide_code_stride(h);
+    ANNB_TRY(ensure_dev((void **)&h->d_wide_codes, &h->cap_wide_codes, (size_t)n_alloc * stride));
+    ANNB_CUDA(cudaMemcpy2DAsync(h->d_wide_codes, stride, raw + g.offset_data, g.size_per_elem, (size_t)d.code_row, (size_t)n,
+                                cudaMemcpyDeviceToDevice, h->stream));
+  }
 
   // labels
   std::vector<uint64_t> labels((size_t)n);
@@ -1136,7 +1180,8 @@ static int search_impl(annb_index *h, const float *queries, const float *tables,
     if (nch > 8) nch = 8;
     if (queries && in_space != ANNB_DEVICE && host_out && plain && nch > 1 && B >= 2 * nch) {
       const size_t TS = (size_t)h->M * h->Ks;
-      const bool fuse = walk4_can_fuse(h);  // the walk builds its own tables: no (B,M,Ks) buffer at all
+      // the walk builds its own tables (or, wide rows, needs none): no (B,M,Ks) buffer at all
+      const bool fuse = walk4_can_fuse(h) || wide_rows(h);
       float *dq, *dtab = nullptr;
       unsigned int *counters;
       int32_t *hfound;
@@ -1204,7 +1249,9 @@ static int search_impl(annb_index *h, const float *queries, const float *tables,
   const double selectivity = has_filter ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
                                            : 1.0 - (double)h->g.num_deleted / (double)std::max<int64_t>(1, h->gd.n);
   // the table is built inside the walk for the plain search (hnsw_walk4) and for the filtered one (hnsw_walk4f)
-  const bool fuse_walk = walk4_can_fuse(h) && (plain_search || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, selectivity)));
+  // (hnsw_walk_wide computes its distances from the queries in every mode)
+  const bool fuse_walk = wide_rows(h) ||
+                         (walk4_can_fuse(h) && (plain_search || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, selectivity))));
   if (tables) {
     ANNB_TRY(stage_in(h, tables, in_space, tbytes, S_TABLES, (const void **)&dt));
   } else if (fuse_walk) {
@@ -1327,11 +1374,15 @@ int annb_scan_subset(annb_index_t *h, const float *queries, int in_space, int64_
     h->n_codes = n;
     float *t = nullptr, *dd = nullptr;
     int64_t *dids = nullptr;
-    if (rc == ANNB_OK) rc = annb_scratch(h, S_TABLES, (size_t)B * h->M * h->Ks * sizeof(float), (void **)&t);
+    const int64_t step = table_chunk_rows(h, B);
+    if (rc == ANNB_OK) rc = annb_scratch(h, S_TABLES, (size_t)std::min(step, B) * h->M * h->Ks * sizeof(float), (void **)&t);
     if (rc == ANNB_OK) rc = annb_scratch(h, S_OUT_L, (size_t)B * k * sizeof(int64_t), (void **)&dids);
     if (rc == ANNB_OK) rc = annb_scratch(h, S_OUT_D, (size_t)B * k * sizeof(float), (void **)&dd);
-    if (rc == ANNB_OK) rc = build_tables(h, queries, in_space, B, normalize, t);
-    if (rc == ANNB_OK) rc = launch_scan_topk(h, t, B, k, dids, dd);
+    for (int64_t b0 = 0; b0 < B && rc == ANNB_OK; b0 += step) {
+      const int64_t nb = std::min(step, B - b0);
+      rc = build_tables(h, queries + (size_t)b0 * h->dim, in_space, nb, normalize, t);
+      if (rc == ANNB_OK) rc = launch_scan_topk(h, t, nb, k, dids + b0 * k, dd + b0 * k);
+    }
     if (rc == ANNB_OK) {
       cudaMemcpyAsync(ids.data(), dids, (size_t)B * k * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream);
       cudaMemcpyAsync(dists_out, dd, (size_t)B * k * sizeof(float), cudaMemcpyDeviceToHost, h->stream);
@@ -1460,7 +1511,7 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   ANNB_TRY(lane_wait(h, lane));  // a lane holds one batch at a time
   const bool host_in = in_space != ANNB_DEVICE, host_out = out_space != ANNB_DEVICE;
   const size_t TS = (size_t)h->M * h->Ks;
-  const bool fuse = walk4_can_fuse(h) && (!general || walk4f_applicable(h, ef_eff, selectivity));
+  const bool fuse = wide_rows(h) || (walk4_can_fuse(h) && (!general || walk4f_applicable(h, ef_eff, selectivity)));
   float *dq = nullptr, *dtab = nullptr, *dd = dists_out;
   uint64_t *dl = labels_out;
   int32_t *dfound;
@@ -1658,6 +1709,15 @@ int annb_sync_counts(annb_index_t *h, int64_t *full_syncs, int64_t *patches) {
   if (!h) ANNB_FAIL(ANNB_EINVAL, "null argument");
   if (full_syncs) *full_syncs = h->full_syncs;
   if (patches) *patches = h->patches;
+  return ANNB_OK;
+}
+
+int annb_device_graph_layout(annb_index_t *h, int64_t *rec0_bytes, int64_t *code_bytes_per_node, int *wide) {
+  if (!h) ANNB_FAIL(ANNB_EINVAL, "null argument");
+  const bool w = wide_rows(h);
+  if (rec0_bytes) *rec0_bytes = h->gd.rec0_bytes;
+  if (code_bytes_per_node) *code_bytes_per_node = w ? wide_code_stride(h) : 0;
+  if (wide) *wide = w ? 1 : 0;
   return ANNB_OK;
 }
 
@@ -2220,14 +2280,14 @@ static int multi_plan(annb_index *h, int64_t B, int ef_eff, const int *query_fil
     const bool general = h->g.num_deleted > 0 || h->opt_force_general;
     g.s = 1.0 - (double)h->g.num_deleted / nn;
     g.mode = general ? (h->opt_force_general == 2 ? 2 : 1) : 0;
-    g.fuse = can_fuse && (!general || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s)));
+    g.fuse = wide_rows(h) || (can_fuse && (!general || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s))));
   }
   for (int i = 1; i < 3; i++) {  // a prepared filter: the filtered route
     MultiGroup &g = grp[i];
     g.filtered = true;
     g.s = smin[i];
     g.mode = h->opt_force_general == 2 ? 2 : 1;
-    g.fuse = can_fuse && h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s);
+    g.fuse = wide_rows(h) || (can_fuse && h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s));
   }
   return ANNB_OK;
 }

@@ -1434,6 +1434,7 @@ int dispatch_flagged(annb_index *h, const SearchParams &p) {
 int launch_search(annb_index *h, const SearchParams &p, int mode) {
   if (p.B == 0) return ANNB_OK;
   if (p.B >= (int64_t)0xffffffffll) ANNB_FAIL(ANNB_ELIMIT, "at most 2^32-2 queries per call");
+  if (wide_rows(h)) return launch_walk_wide(h, p);  // every mode: the literal walk, table-free (walk_wide.cu)
   if (mode == 1) {  // filter and/or deletions: two register lists in hnsw_walk4's mapping where that applies (walk_flagged4.cu)
     const int rc = launch_walk4f(h, p);
     if (rc != 1) return rc;
@@ -1473,8 +1474,9 @@ int launch_search(annb_index *h, const SearchParams &p, int mode) {
 int launch_pack_rec0(annb_index *h, const uint8_t *d_level0_raw, int64_t n) {
   if (n == 0) return ANNB_OK;
   const int64_t total = n * h->gd.maxM0;
+  const int code_row = wide_rows(h) ? 0 : h->gd.code_row;  // wide rows: links-only records
   pack_rec0_kernel<<<(unsigned)((total + 255) / 256), 256, 0, h->stream>>>(
-      d_level0_raw, n, (int)h->g.size_per_elem, (int)h->g.offset_data, h->gd.maxM0, h->gd.code_row, h->gd.code_off0,
+      d_level0_raw, n, (int)h->g.size_per_elem, (int)h->g.offset_data, h->gd.maxM0, code_row, h->gd.code_off0,
       h->gd.rec0_bytes,
       h->d_rec0);
   h->launches++;

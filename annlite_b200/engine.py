@@ -469,6 +469,14 @@ class Engine:
         L.check(self._lib.annb_sync_counts(self._h, C.byref(a), C.byref(b)))
         return a.value, b.value
 
+    @property
+    def device_graph_layout(self):
+        """(level-0 record bytes per node, own code-row bytes per node, wide) of the device graph as the last search
+        laid it out; wide code rows (> 128 bytes) store links only in the records and each code row once."""
+        r, c, w = C.c_int64(), C.c_int64(), C.c_int()
+        L.check(self._lib.annb_device_graph_layout(self._h, C.byref(r), C.byref(c), C.byref(w)))
+        return r.value, c.value, bool(w.value)
+
     def set_option(self, name, value):
         L.check(self._lib.annb_set_option(self._h, name.encode(), int(value)))
 

@@ -61,6 +61,13 @@ extern "C" {
 
 #define ANNB_MAX_EF 512 /* top-candidate list lives in registers: 16 entries x 32 lanes */
 
+/* Widest PQ code row (n_subvectors x code bytes) an index may have: M = 768 one-byte codes or M = 512 two-byte codes
+ * (ANNB_ELIMIT beyond).  Rows of up to 128 bytes are stored next to each neighbour link on the device and searched by
+ * the table kernels; wider rows are stored once per node and searched by hnsw_walk_wide, which computes each
+ * distance from the query and the codebook instead of a per-query table (DESIGN.md sections 3-4). */
+#define ANNB_MAX_CODE_ROW 1024
+#define ANNB_NARROW_CODE_ROW 128
+
 typedef struct annb_index annb_index_t;
 
 /* ---- library / error -------------------------------------------------------------------- */
@@ -489,6 +496,10 @@ ANNB_API int annb_fallback_queries(annb_index_t *h, int64_t *out);
  * a small host insertion rewrote were uploaded (the reference searches the structure it inserts into: hnswalg.h:1108;
  * here insertions happen on the host graph and the walk layout on the device follows). */
 ANNB_API int annb_sync_counts(annb_index_t *h, int64_t *full_syncs, int64_t *patches);
+/* Bytes per node of the device graph as the last search laid it out: the level-0 walk record (links, plus the
+ * neighbours' codes for code rows of <= 128 bytes) and the node's own code row in the by-id code matrix (wide code
+ * rows only, 16-byte aligned; 0 otherwise).  *wide = 1 when the index takes the wide-row layout and hnsw_walk_wide. */
+ANNB_API int annb_device_graph_layout(annb_index_t *h, int64_t *rec0_bytes, int64_t *code_bytes_per_node, int *wide);
 /* Tuning / A-B / test switches (none changes results): "chunks" (host-buffer pipeline depth of annb_search, 1 = off),
  * "walk_kernel" (plain search: 0 hnsw_walk4 fused, 2 hnsw_walk4 over K1 tables, 1 round-1 kernels), "flagged_kernel"
  * (filter / deletions: 0 hnsw_walk4f where it applies, 1 hnsw_walk_flagged), "flagged_en" (force hnsw_walk4f's
