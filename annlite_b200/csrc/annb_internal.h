@@ -227,23 +227,31 @@ struct SubsetScan {
   int32_t nq, k, cell, pad;
 };
 
-// a batch with one filter per query (annb_search_multi / annb_search_submit_multi), in its gathered row order: the
-// rows of each routing group are contiguous; gathered row i is the caller's row perm[i]
+// An enqueued search batch, as its flagged queries (found = -1) are re-run on the bitmap walk (capi.cu: rerun_flagged).
+// A batch with one filter per query (annb_search_multi / annb_search_submit_multi) is in its gathered row order: the
+// rows of each routing group are contiguous; gathered row i is the caller's row dperm[i].  dperm == nullptr: the rows
+// are in the caller's order and the gathered outputs are the caller's.
 struct MultiBatch {
   int64_t B = 0;
   int k = 0, ef = 0;
   const float *dq = nullptr;                 // gathered queries, normalised (B, dim)
-  const uint32_t *const *dqf = nullptr;      // gathered per-query bitmaps (nullptr = no filter)
-  const uint32_t *dperm = nullptr;           // (B) caller row of each gathered row
+  const uint32_t *filter = nullptr;          // by-id bitmap of every row (nullptr = none) ...
+  float selectivity = 1.f;                   // ... and the fraction of nodes it admits
+  const uint32_t *const *dqf = nullptr;      // gathered per-query bitmaps (nullptr = no filter), or nullptr
+  const uint32_t *dperm = nullptr;           // (B) caller row of each gathered row, or nullptr
   uint64_t *gl = nullptr;                    // gathered outputs (B, k) / (B, k) / (B)
   float *gd = nullptr;
   int32_t *gfound = nullptr;
+  int64_t *gstats = nullptr;                 // (B, 3) counters (annb_search), or nullptr
   uint64_t *dl = nullptr;                    // outputs in the caller's row order, on the device
   float *dd = nullptr;
   uint64_t *host_labels = nullptr;           // host outputs, or nullptr (device outputs)
   float *host_dists = nullptr;
+  int64_t *host_stats = nullptr;
   int32_t *hfound = nullptr;                 // pinned copy of gfound
-  int table_slot = 0;                        // scratch slot of the K1 tables a re-run builds
+  const float *tables = nullptr;             // K1 tables a re-run reuses, or nullptr: it builds them from dq ...
+  int table_slot = 0;                        // ... in this scratch slot
+  bool timing = false;                       // a re-run records ev[2] / ev[3] around its launch (annb_last_kernel_ms)
 };
 
 // ------------------------------------------------------------------------------------------
@@ -297,22 +305,8 @@ struct annb_index {
   // asynchronous submit/wait lanes (annb_search_submit): lane i works on stream i with its own scratch
   struct AsyncLane {
     bool busy = false;
-    int64_t B = 0;
-    int k = 0;
-    int32_t *hfound = nullptr;
-    // what a filtered / deletion-aware batch needs to re-run its flagged queries at wait time
-    bool flagged = false;
-    int ef = 0;
-    const float *dq = nullptr;          // device queries (normalised), valid until the lane's next submit
-    const uint32_t *dfilter = nullptr;  // by-id filter bitmap or nullptr
-    float selectivity = 1.f;
-    uint64_t *dl = nullptr;
-    float *dd = nullptr;
-    int32_t *dfound = nullptr;
-    uint64_t *host_labels = nullptr;    // host outputs to refresh after a re-run, or nullptr (device outputs)
-    float *host_dists = nullptr;
-    bool multi = false;                 // a per-query filter batch (annb_search_submit_multi): its state is `mb`
-    MultiBatch mb;
+    bool flagged = false;  // a filtered / deletion-aware batch: its flagged queries are re-run at wait time
+    MultiBatch batch;      // its buffers stay valid until the lane's next submit
   } lanes[2];
   uint32_t next_ticket = 0;
 

@@ -246,7 +246,7 @@ int annb_stream(annb_index_t *h, uint64_t *stream_out) {
 }
 
 static int lane_wait(annb_index *h, int lane);
-static int lane_rerun_flagged(annb_index *h, int lane, int64_t n_over);
+static int lane_finish(annb_index *h, int lane, bool check);
 
 // A streamed filtered batch whose walk flagged queries is finished (those queries re-run on the bitmap walk) out of
 // the lane's own scratch: queries, filter bitmap, device outputs.  Lane 0 shares these buffers with the blocking entry
@@ -257,9 +257,7 @@ static int settle_flagged_lanes(annb_index *h) {
     annb_index::AsyncLane &L = h->lanes[lane];
     if (!L.busy || !L.flagged) continue;
     ANNB_CUDA(cudaStreamSynchronize(lane ? h->stream2 : h->stream));
-    int64_t n_over = 0;
-    for (int64_t b = 0; b < L.B; b++) n_over += L.hfound[b] < 0;
-    if (n_over) ANNB_TRY(lane_rerun_flagged(h, lane, n_over));
+    ANNB_TRY(lane_finish(h, lane, false));
     L.flagged = false;
   }
   return ANNB_OK;
@@ -1110,11 +1108,28 @@ int annb_search(annb_index_t *h, const float *queries, const float *tables, int 
 
 }  // extern "C"
 
-// a label list -> the by-id bitmap of the rows it names ((gd.n + 31) / 32 + 1 words), on the handle's stream
-static int labels_to_bitmap(annb_index *h, const uint64_t *filter_labels, int filter_space, int64_t n_filter, uint32_t *by_id) {
-  if (h->max_label > (uint64_t)h->gd.n * 64 + (1ull << 30)) {
-    // labels too sparse for a by-label bitmap on the device: resolve them through the host's
-    // label -> internal id map (the same map mark_deleted uses) and upload the by-id bitmap
+// labels too sparse for a by-label bitmap on the device: labels_to_bitmap resolves them on the host
+static bool sparse_labels(const annb_index *h) { return h->max_label > (uint64_t)h->gd.n * 64 + (1ull << 30); }
+
+// labels_to_bitmap's staging buffers in lane `lane`'s scratch: the by-label bitmap and the device copy of host labels
+// (*staged = nullptr for device labels; neither for sparse labels)
+static int label_staging(annb_index *h, int lane, int filter_space, int64_t n_filter, uint64_t **staged, uint32_t **by_label) {
+  *staged = nullptr;
+  *by_label = nullptr;
+  if (sparse_labels(h)) return ANNB_OK;
+  ANNB_TRY(annb_scratch(h, lane ? S_L1_FLT_BY_LABEL : S_FLT_BY_LABEL, ((size_t)(h->max_label >> 5) + 1) * 4, (void **)by_label));
+  if (filter_space != ANNB_DEVICE)
+    ANNB_TRY(annb_scratch(h, lane ? S_L1_FLT_LABELS : S_FLT_LABELS, (size_t)std::max<int64_t>(n_filter, 1) * 8, (void **)staged));
+  return ANNB_OK;
+}
+
+// a label list -> the by-id bitmap of the rows it names ((gd.n + 31) / 32 + 1 words), on h->stream, through the
+// staging buffers of label_staging
+static int labels_to_bitmap(annb_index *h, const uint64_t *filter_labels, int filter_space, int64_t n_filter, uint64_t *staged,
+                            uint32_t *by_label, uint32_t *by_id) {
+  if (sparse_labels(h)) {
+    // resolve the labels through the host's label -> internal id map (the same map mark_deleted uses) and upload the
+    // by-id bitmap
     std::vector<uint64_t> tmp;
     const uint64_t *hl = filter_labels;
     if (filter_space == ANNB_DEVICE) {
@@ -1130,13 +1145,86 @@ static int labels_to_bitmap(annb_index *h, const uint64_t *filter_labels, int fi
     }
     ANNB_CUDA(cudaMemcpyAsync(by_id, bm.data(), bm.size() * 4, cudaMemcpyHostToDevice, h->stream));
     ANNB_CUDA(cudaStreamSynchronize(h->stream));
-  } else {
-    const uint64_t *dfl;
-    ANNB_TRY(stage_in(h, filter_labels, filter_space, (size_t)std::max<int64_t>(n_filter, 1) * 8, S_FLT_LABELS, (const void **)&dfl));
-    uint32_t *by_label;
-    ANNB_TRY(annb_scratch(h, S_FLT_BY_LABEL, ((size_t)(h->max_label >> 5) + 1) * 4, (void **)&by_label));
-    ANNB_TRY(launch_filter_bitmap(h, dfl, n_filter, by_label, by_id));
+    return ANNB_OK;
   }
+  const uint64_t *dfl = filter_labels;
+  if (staged) {
+    ANNB_CUDA(cudaMemcpyAsync(staged, filter_labels, (size_t)n_filter * 8, cudaMemcpyHostToDevice, h->stream));
+    dfl = staged;
+  }
+  return launch_filter_bitmap(h, dfl, n_filter, by_label, by_id);
+}
+
+// A batch's walk outputs scattered to the caller's rows (dperm), then `found` and the host outputs copied back, on
+// h->stream
+static int batch_outputs(annb_index *h, const MultiBatch &mb) {
+  if (mb.dperm) {
+    ANNB_TRY(launch_rows_copy(h, mb.gl, mb.dl, mb.dperm, mb.B, 2 * mb.k, true));
+    ANNB_TRY(launch_rows_copy(h, mb.gd, mb.dd, mb.dperm, mb.B, mb.k, true));
+  }
+  ANNB_CUDA(cudaMemcpyAsync(mb.hfound, mb.gfound, (size_t)mb.B * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (mb.host_labels) {
+    ANNB_CUDA(cudaMemcpyAsync(mb.host_labels, mb.dl, (size_t)mb.B * mb.k * 8, cudaMemcpyDeviceToHost, h->stream));
+    ANNB_CUDA(cudaMemcpyAsync(mb.host_dists, mb.dd, (size_t)mb.B * mb.k * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (mb.host_stats) ANNB_CUDA(cudaMemcpyAsync(mb.host_stats, mb.gstats, (size_t)mb.B * 24, cudaMemcpyDeviceToHost, h->stream));
+  }
+  return ANNB_OK;
+}
+
+// The queries of a settled batch that outgrew the flagged walk's list (found = -1, n_over of them) re-run on the bitmap
+// walk (exact, any size) through a query-row map, with their own bitmaps, on h->stream: only their rows of the outputs
+// are overwritten, then the outputs are copied back again.
+static int rerun_flagged(annb_index *h, MultiBatch &mb, int64_t n_over) {
+  uint32_t *hmap, *dmap;
+  ANNB_TRY(annb_pinned(h, 3, (size_t)n_over * 4, (void **)&hmap));
+  ANNB_TRY(annb_scratch(h, S_QMAP, (size_t)n_over * 4, (void **)&dmap));
+  const float *tables = mb.tables;
+  float *t = nullptr;
+  if (!tables) ANNB_TRY(annb_scratch(h, mb.table_slot, (size_t)mb.B * h->M * h->Ks * sizeof(float), (void **)&t));
+  int64_t w = 0;
+  for (int64_t b = 0; b < mb.B; b++)
+    if (mb.hfound[b] < 0) hmap[w++] = (uint32_t)b;
+  ANNB_CUDA(cudaMemcpyAsync(dmap, hmap, (size_t)n_over * 4, cudaMemcpyHostToDevice, h->stream));
+  if (!tables) {  // the walk built its tables in shared memory: the bitmap walk reads them from HBM (K1, all rows)
+    ANNB_TRY(launch_adc_table(h, mb.dq, mb.B, t));
+    tables = t;
+  }
+  SearchParams p;
+  memset(&p, 0, sizeof(p));
+  p.tables = tables;
+  p.B = n_over;
+  p.k = mb.k;
+  p.ef = mb.ef;
+  p.filter = mb.filter;
+  p.query_filter = mb.dqf;
+  p.selectivity = mb.selectivity;
+  p.out_labels = mb.gl;
+  p.out_dists = mb.gd;
+  p.out_found = mb.gfound;
+  p.out_stats = mb.gstats;
+  p.qmap = dmap;
+  if (mb.timing && h->opt_timing) cudaEventRecord(h->ev[2], h->stream);
+  ANNB_TRY(launch_search(h, p, 2));
+  if (mb.timing && h->opt_timing) cudaEventRecord(h->ev[3], h->stream);
+  ANNB_TRY(batch_outputs(h, mb));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  h->flagged_fallbacks++;
+  h->flagged_fallback_queries += n_over;
+  return ANNB_OK;
+}
+
+// A settled batch: its flagged queries re-run (`flagged` = its walks can flag queries), then (check) ANNB_EFEWRESULTS
+// where a query has fewer than k results (hnsw_bindings.cpp:342-345)
+static int finish_batch(annb_index *h, MultiBatch &mb, bool flagged, bool check) {
+  if (flagged) {
+    int64_t n_over = 0;
+    for (int64_t b = 0; b < mb.B; b++) n_over += mb.hfound[b] < 0;
+    if (n_over) ANNB_TRY(rerun_flagged(h, mb, n_over));
+  }
+  if (check)
+    for (int64_t b = 0; b < mb.B; b++)
+      if (mb.hfound[b] < mb.k)
+        ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   return ANNB_OK;
 }
 
@@ -1267,9 +1355,11 @@ static int search_impl(annb_index *h, const float *queries, const float *tables,
   if (pf) {
     dfilter = pf->bits;
   } else if (filter_labels) {
-    uint32_t *by_id;
+    uint32_t *by_id, *by_label;
+    uint64_t *staged;
     ANNB_TRY(annb_scratch(h, S_FLT_BY_ID, ((size_t)(h->gd.n + 31) / 32 + 1) * 4, (void **)&by_id));
-    ANNB_TRY(labels_to_bitmap(h, filter_labels, filter_space, n_filter, by_id));
+    ANNB_TRY(label_staging(h, 0, filter_space, n_filter, &staged, &by_label));
+    ANNB_TRY(labels_to_bitmap(h, filter_labels, filter_space, n_filter, staged, by_label, by_id));
     dfilter = by_id;
   }
   SearchParams p;
@@ -1287,51 +1377,31 @@ static int search_impl(annb_index *h, const float *queries, const float *tables,
   p.out_stats = dstats;
   const bool general = dfilter != nullptr || h->g.num_deleted > 0 || h->opt_force_general;
   p.selectivity = (float)selectivity;
-  int32_t *hfound;
-  ANNB_TRY(annb_pinned(h, 2, (size_t)B * 4, (void **)&hfound));
-  int mode = general ? (h->opt_force_general == 2 ? 2 : 1) : 0;
-  for (;;) {
-    if (h->opt_timing) cudaEventRecord(h->ev[2], h->stream);
-    ANNB_TRY(launch_search(h, p, mode));
-    if (h->opt_timing) cudaEventRecord(h->ev[3], h->stream);
-    // found < k anywhere?  (hnsw_bindings.cpp:342-345).  A tiny reduction on the host side of `found`.
-    ANNB_CUDA(cudaMemcpyAsync(hfound, dfound, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
-    if (host_out) {
-      ANNB_CUDA(cudaMemcpyAsync(labels_out, dl, (size_t)B * k * 8, cudaMemcpyDeviceToHost, h->stream));
-      ANNB_CUDA(cudaMemcpyAsync(dists_out, dd, (size_t)B * k * 4, cudaMemcpyDeviceToHost, h->stream));
-      if (stats_out) ANNB_CUDA(cudaMemcpyAsync(stats_out, dstats, (size_t)B * 24, cudaMemcpyDeviceToHost, h->stream));
-    }
-    ANNB_CUDA(cudaStreamSynchronize(h->stream));
-    if (mode == 2) break;
-    // queries that outgrew the flagged walk's list (found = -1): only those are redone on the bitmap walk
-    // (exact, any size) through a query-index map; their rows of the outputs are simply overwritten
-    int64_t n_over = 0;
-    for (int64_t b = 0; b < B; b++) n_over += hfound[b] < 0;
-    if (n_over == 0) break;
-    uint32_t *hmap, *dmap;
-    ANNB_TRY(annb_pinned(h, 3, (size_t)n_over * 4, (void **)&hmap));
-    ANNB_TRY(annb_scratch(h, S_QMAP, (size_t)n_over * 4, (void **)&dmap));
-    int64_t w = 0;
-    for (int64_t b = 0; b < B; b++)
-      if (hfound[b] < 0) hmap[w++] = (uint32_t)b;
-    ANNB_CUDA(cudaMemcpyAsync(dmap, hmap, (size_t)n_over * 4, cudaMemcpyHostToDevice, h->stream));
-    if (!p.tables) {  // the walk built its tables in shared memory: the bitmap walk reads them from HBM (K1, all rows)
-      float *t;
-      ANNB_TRY(annb_scratch(h, S_TABLES, tbytes, (void **)&t));
-      ANNB_TRY(launch_adc_table(h, p.queries, B, t));
-      p.tables = t;
-      p.queries = nullptr;
-    }
-    p.qmap = dmap;
-    p.B = n_over;
-    mode = 2;
-    h->flagged_fallbacks++;
-    h->flagged_fallback_queries += n_over;
-  }
-  for (int64_t b = 0; b < B; b++)
-    if (hfound[b] < k)
-      ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
-  return ANNB_OK;
+  MultiBatch mb;
+  mb.B = B;
+  mb.k = k;
+  mb.ef = ef_eff;
+  mb.dq = p.queries;
+  mb.filter = dfilter;
+  mb.selectivity = p.selectivity;
+  mb.gl = mb.dl = dl;
+  mb.gd = mb.dd = dd;
+  mb.gfound = dfound;
+  mb.gstats = dstats;
+  mb.host_labels = host_out ? labels_out : nullptr;
+  mb.host_dists = host_out ? dists_out : nullptr;
+  mb.host_stats = host_out ? stats_out : nullptr;
+  mb.tables = p.tables;
+  mb.table_slot = S_TABLES;
+  mb.timing = true;
+  ANNB_TRY(annb_pinned(h, 2, (size_t)B * 4, (void **)&mb.hfound));
+  const int mode = general ? (h->opt_force_general == 2 ? 2 : 1) : 0;
+  if (h->opt_timing) cudaEventRecord(h->ev[2], h->stream);
+  ANNB_TRY(launch_search(h, p, mode));
+  if (h->opt_timing) cudaEventRecord(h->ev[3], h->stream);
+  ANNB_TRY(batch_outputs(h, mb));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  return finish_batch(h, mb, mode != 2, true);
 }
 
 extern "C" {
@@ -1410,77 +1480,21 @@ int annb_scan_subset(annb_index_t *h, const float *queries, int in_space, int64_
 // ---- streaming submit / wait ---------------------------------------------------------------------
 // A filtered / deletion-aware batch whose walk flagged queries (found = -1: N outgrew its capacity) is finished at
 // wait time: exactly those queries are re-run on the bitmap walk, on the lane's own stream and scratch.
-static int multi_rerun(annb_index *h, MultiBatch &mb, int64_t n_over);
-
-static int lane_rerun_flagged(annb_index *h, int lane, int64_t n_over) {
+static int lane_finish(annb_index *h, int lane, bool check) {
   annb_index::AsyncLane &L = h->lanes[lane];
-  cudaStream_t st = lane ? h->stream2 : h->stream;
-  if (L.multi) {
-    cudaStream_t saved = h->stream;
-    h->stream = st;
-    const int rc = multi_rerun(h, L.mb, n_over);
-    h->stream = saved;
-    return rc;
-  }
-  uint32_t *hmap, *dmap;
-  float *t;
-  ANNB_TRY(annb_pinned(h, 3, (size_t)n_over * 4, (void **)&hmap));
-  ANNB_TRY(annb_scratch(h, S_QMAP, (size_t)n_over * 4, (void **)&dmap));
-  ANNB_TRY(annb_scratch(h, lane ? S_L1_TABLES : S_TABLES, (size_t)L.B * h->M * h->Ks * sizeof(float), (void **)&t));
-  int64_t w = 0;
-  for (int64_t b = 0; b < L.B; b++)
-    if (L.hfound[b] < 0) hmap[w++] = (uint32_t)b;
   cudaStream_t saved = h->stream;
-  h->stream = st;
-  int rc = ANNB_OK;
-  if (cudaMemcpyAsync(dmap, hmap, (size_t)n_over * 4, cudaMemcpyHostToDevice, st) != cudaSuccess) rc = ANNB_ECUDA;
-  if (rc == ANNB_OK) rc = launch_adc_table(h, L.dq, L.B, t);
-  if (rc == ANNB_OK) {
-    SearchParams p;
-    memset(&p, 0, sizeof(p));
-    p.tables = t;
-    p.B = n_over;
-    p.k = L.k;
-    p.ef = L.ef;
-    p.filter = L.dfilter;
-    p.selectivity = L.selectivity;
-    p.out_labels = L.dl;
-    p.out_dists = L.dd;
-    p.out_found = L.dfound;
-    p.qmap = dmap;
-    rc = launch_search(h, p, 2);
-  }
-  if (rc == ANNB_OK) {
-    cudaMemcpyAsync(L.hfound, L.dfound, (size_t)L.B * 4, cudaMemcpyDeviceToHost, st);
-    if (L.host_labels) {
-      cudaMemcpyAsync(L.host_labels, L.dl, (size_t)L.B * L.k * 8, cudaMemcpyDeviceToHost, st);
-      cudaMemcpyAsync(L.host_dists, L.dd, (size_t)L.B * L.k * 4, cudaMemcpyDeviceToHost, st);
-    }
-    if (cudaStreamSynchronize(st) != cudaSuccess) rc = ANNB_ECUDA;
-  }
+  h->stream = lane ? h->stream2 : saved;
+  const int rc = finish_batch(h, L.batch, L.flagged, check);
   h->stream = saved;
-  if (rc == ANNB_ECUDA) annb_set_error("CUDA error while re-running flagged queries of a streamed search: %s", cudaGetErrorString(cudaGetLastError()));
-  if (rc != ANNB_OK) return rc;
-  h->flagged_fallbacks++;
-  h->flagged_fallback_queries += n_over;
-  return ANNB_OK;
+  return rc;
 }
 
 static int lane_wait(annb_index *h, int lane) {
   annb_index::AsyncLane &L = h->lanes[lane];
   if (!L.busy) return ANNB_OK;
-  cudaStream_t st = lane ? h->stream2 : h->stream;
-  ANNB_CUDA(cudaStreamSynchronize(st));
+  ANNB_CUDA(cudaStreamSynchronize(lane ? h->stream2 : h->stream));
   L.busy = false;
-  if (L.flagged) {
-    int64_t n_over = 0;
-    for (int64_t b = 0; b < L.B; b++) n_over += L.hfound[b] < 0;
-    if (n_over) ANNB_TRY(lane_rerun_flagged(h, lane, n_over));
-  }
-  for (int64_t b = 0; b < L.B; b++)
-    if (L.hfound[b] < L.k)
-      ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
-  return ANNB_OK;
+  return lane_finish(h, lane, true);
 }
 
 // one batch, enqueued entirely on one lane: H2D -> normalise -> [filter bitmap] -> walk (tables built inside) -> D2H
@@ -1505,7 +1519,6 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   const bool general = filter_labels != nullptr || pf || h->g.num_deleted > 0 || h->opt_force_general;
   const double selectivity = (filter_labels || pf) ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
                                                    : 1.0 - (double)h->g.num_deleted / (double)std::max<int64_t>(1, h->gd.n);
-  const bool sparse_labels = h->max_label > (uint64_t)h->gd.n * 64 + (1ull << 30);
   const int ticket = (int)(h->next_ticket++ & 0x3fffffff);
   const int lane = ticket & 1;
   ANNB_TRY(lane_wait(h, lane));  // a lane holds one batch at a time
@@ -1530,14 +1543,21 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   ANNB_TRY(annb_scratch(h, S_LANE_COUNTERS, 512, (void **)&counters));
   if (filter_labels) {
     ANNB_TRY(annb_scratch(h, lane ? S_L1_FLT_BY_ID : S_FLT_BY_ID, ((size_t)(h->gd.n + 31) / 32 + 1) * 4, (void **)&by_id));
-    if (!sparse_labels) {
-      ANNB_TRY(annb_scratch(h, lane ? S_L1_FLT_BY_LABEL : S_FLT_BY_LABEL, ((size_t)(h->max_label >> 5) + 1) * 4, (void **)&by_label));
-      if (filter_space != ANNB_DEVICE)
-        ANNB_TRY(annb_scratch(h, lane ? S_L1_FLT_LABELS : S_FLT_LABELS, (size_t)std::max<int64_t>(n_filter, 1) * 8, (void **)&dflt));
-    }
+    ANNB_TRY(label_staging(h, lane, filter_space, n_filter, &dflt, &by_label));
   }
-  int32_t *hfound;
-  ANNB_TRY(annb_pinned(h, 4 + lane, (size_t)B * 4, (void **)&hfound));
+  MultiBatch mb;
+  ANNB_TRY(annb_pinned(h, 4 + lane, (size_t)B * 4, (void **)&mb.hfound));
+  mb.B = B;
+  mb.k = k;
+  mb.ef = ef_eff;
+  mb.filter = by_id;
+  mb.selectivity = (float)selectivity;
+  mb.gl = mb.dl = dl;
+  mb.gd = mb.dd = dd;
+  mb.gfound = dfound;
+  mb.host_labels = host_out ? labels_out : nullptr;
+  mb.host_dists = host_out ? dists_out : nullptr;
+  mb.table_slot = lane ? S_L1_TABLES : S_TABLES;
 
   cudaStream_t saved = h->stream;
   h->stream = lane ? h->stream2 : saved;
@@ -1549,34 +1569,9 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
       rc = ANNB_ECUDA;
     src = dq;
   }
+  mb.dq = src;
   for (int r = 0; r < normalize && rc == ANNB_OK; r++) rc = launch_l2_normalize(h, dq, B, h->dim);
-  if (rc == ANNB_OK && filter_labels) {
-    if (sparse_labels) {
-      // labels too sparse for a by-label bitmap on the device: resolve them through the host's label -> id map
-      std::vector<uint64_t> tmp;
-      const uint64_t *hl = filter_labels;
-      if (filter_space == ANNB_DEVICE) {
-        tmp.resize((size_t)n_filter);
-        if (cudaMemcpy(tmp.data(), filter_labels, (size_t)n_filter * 8, cudaMemcpyDeviceToHost) != cudaSuccess) rc = ANNB_ECUDA;
-        hl = tmp.data();
-      }
-      std::vector<uint32_t> bm((size_t)(h->gd.n + 31) / 32 + 1, 0u);
-      for (int64_t i = 0; i < n_filter && rc == ANNB_OK; i++) {
-        auto it = h->g.label_lookup.find(hl[i]);
-        if (it != h->g.label_lookup.end()) bm[it->second >> 5] |= 1u << (it->second & 31);
-      }
-      if (rc == ANNB_OK && (cudaMemcpyAsync(by_id, bm.data(), bm.size() * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-                            cudaStreamSynchronize(h->stream) != cudaSuccess))
-        rc = ANNB_ECUDA;
-    } else {
-      const uint64_t *dfl = filter_labels;
-      if (dflt) {
-        if (cudaMemcpyAsync(dflt, filter_labels, (size_t)n_filter * 8, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) rc = ANNB_ECUDA;
-        dfl = dflt;
-      }
-      if (rc == ANNB_OK) rc = launch_filter_bitmap(h, dfl, n_filter, by_label, by_id);
-    }
-  }
+  if (rc == ANNB_OK && filter_labels) rc = labels_to_bitmap(h, filter_labels, filter_space, n_filter, dflt, by_label, by_id);
   if (rc == ANNB_OK && !fuse) rc = launch_adc_table(h, src, B, dtab);
   if (rc == ANNB_OK) {
     SearchParams p;
@@ -1594,14 +1589,7 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
     p.selectivity = (float)selectivity;
     rc = launch_search(h, p, general ? 1 : 0);
   }
-  if (rc == ANNB_OK) {
-    cudaMemcpyAsync(hfound, dfound, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream);
-    if (host_out) {
-      cudaMemcpyAsync(labels_out, dl, (size_t)B * k * 8, cudaMemcpyDeviceToHost, h->stream);
-      cudaMemcpyAsync(dists_out, dd, (size_t)B * k * 4, cudaMemcpyDeviceToHost, h->stream);
-    }
-    if (cudaGetLastError() != cudaSuccess) rc = ANNB_ECUDA;
-  }
+  if (rc == ANNB_OK) rc = batch_outputs(h, mb);
   h->stream = saved;
   if (rc != ANNB_OK) {
     if (rc == ANNB_ECUDA) annb_set_error("CUDA error while enqueuing a streamed search");
@@ -1609,20 +1597,8 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   }
   annb_index::AsyncLane &L = h->lanes[lane];
   L.busy = true;
-  L.B = B;
-  L.k = k;
-  L.hfound = hfound;
   L.flagged = general;
-  L.ef = ef_eff;
-  L.dq = src;
-  L.dfilter = by_id;
-  L.selectivity = (float)selectivity;
-  L.dl = dl;
-  L.dd = dd;
-  L.dfound = dfound;
-  L.host_labels = host_out ? labels_out : nullptr;
-  L.host_dists = host_out ? dists_out : nullptr;
-  L.multi = false;
+  L.batch = mb;
   *ticket_out = ticket;
   return ANNB_OK;
 }
@@ -2150,13 +2126,16 @@ int annb_filter_prepare_labels(annb_index_t *h, const uint64_t *labels, int64_t 
     auto it = h->g.label_lookup.find(lab[i]);
     if (it != h->g.label_lookup.end() && !h->g.deleted(it->second)) ids.push_back(it->second);
   }
+  uint64_t *staged;
+  uint32_t *by_label;
+  ANNB_TRY(label_staging(h, 0, space, n, &staged, &by_label));
   void *block = nullptr;
   ANNB_CUDA(cudaMalloc(&block, (words + ids.size()) * 4));
   std::shared_ptr<void> owner(block, [](void *p) { cudaFree(p); });
   uint32_t *bits = (uint32_t *)block;
   ANNB_CUDA(cudaMemsetAsync(bits, 0, words * 4, h->stream));
   if (!ids.empty()) ANNB_CUDA(cudaMemcpyAsync(bits + words, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, h->stream));
-  ANNB_TRY(labels_to_bitmap(h, labels, space, n, bits));
+  ANNB_TRY(labels_to_bitmap(h, labels, space, n, staged, by_label, bits));
   ANNB_CUDA(cudaStreamSynchronize(h->stream));
   PreparedFilter pf;
   pf.bits = bits;
@@ -2376,65 +2355,9 @@ static int multi_enqueue(annb_index *h, int lane, const float *queries, int in_s
     rc = launch_search(h, p, g.mode);
   }
   if (rc == ANNB_OK && timing) cudaEventRecord(h->ev[3], h->stream);
-  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gl, dl, mb.dperm, B, 2 * k, true);
-  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gd, dd, mb.dperm, B, k, true);
-  if (rc == ANNB_OK) {
-    cudaMemcpyAsync(hfound, mb.gfound, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream);
-    if (host_out) {
-      cudaMemcpyAsync(labels_out, dl, (size_t)B * k * 8, cudaMemcpyDeviceToHost, h->stream);
-      cudaMemcpyAsync(dists_out, dd, (size_t)B * k * 4, cudaMemcpyDeviceToHost, h->stream);
-    }
-    if (cudaGetLastError() != cudaSuccess) rc = ANNB_ECUDA;
-  }
+  if (rc == ANNB_OK) rc = batch_outputs(h, mb);
   if (rc == ANNB_ECUDA) annb_set_error("CUDA error while enqueuing a per-query filter search: %s", cudaGetErrorString(cudaGetLastError()));
   return rc;
-}
-
-// the flagged queries of a settled batch (found = -1) re-run on the bitmap walk with their own bitmaps, on h->stream;
-// then the outputs are scattered and copied back again
-static int multi_rerun(annb_index *h, MultiBatch &mb, int64_t n_over) {
-  uint32_t *hmap, *dmap;
-  float *t;
-  ANNB_TRY(annb_pinned(h, 3, (size_t)n_over * 4, (void **)&hmap));
-  ANNB_TRY(annb_scratch(h, S_QMAP, (size_t)n_over * 4, (void **)&dmap));
-  ANNB_TRY(annb_scratch(h, mb.table_slot, (size_t)mb.B * h->M * h->Ks * sizeof(float), (void **)&t));
-  int64_t w = 0;
-  for (int64_t b = 0; b < mb.B; b++)
-    if (mb.hfound[b] < 0) hmap[w++] = (uint32_t)b;
-  int rc = ANNB_OK;
-  if (cudaMemcpyAsync(dmap, hmap, (size_t)n_over * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) rc = ANNB_ECUDA;
-  if (rc == ANNB_OK) rc = launch_adc_table(h, mb.dq, mb.B, t);
-  if (rc == ANNB_OK) {
-    SearchParams p;
-    memset(&p, 0, sizeof(p));
-    p.tables = t;
-    p.B = n_over;
-    p.k = mb.k;
-    p.ef = mb.ef;
-    p.query_filter = mb.dqf;
-    p.selectivity = 1.f;
-    p.out_labels = mb.gl;
-    p.out_dists = mb.gd;
-    p.out_found = mb.gfound;
-    p.qmap = dmap;
-    rc = launch_search(h, p, 2);
-  }
-  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gl, mb.dl, mb.dperm, mb.B, 2 * mb.k, true);
-  if (rc == ANNB_OK) rc = launch_rows_copy(h, mb.gd, mb.dd, mb.dperm, mb.B, mb.k, true);
-  if (rc == ANNB_OK) {
-    cudaMemcpyAsync(mb.hfound, mb.gfound, (size_t)mb.B * 4, cudaMemcpyDeviceToHost, h->stream);
-    if (mb.host_labels) {
-      cudaMemcpyAsync(mb.host_labels, mb.dl, (size_t)mb.B * mb.k * 8, cudaMemcpyDeviceToHost, h->stream);
-      cudaMemcpyAsync(mb.host_dists, mb.dd, (size_t)mb.B * mb.k * 4, cudaMemcpyDeviceToHost, h->stream);
-    }
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess) rc = ANNB_ECUDA;
-  }
-  if (rc == ANNB_ECUDA) annb_set_error("CUDA error while re-running flagged queries of a per-query filter search: %s",
-                                       cudaGetErrorString(cudaGetLastError()));
-  if (rc != ANNB_OK) return rc;
-  h->flagged_fallbacks++;
-  h->flagged_fallback_queries += n_over;
-  return ANNB_OK;
 }
 
 int annb_search_multi(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
@@ -2460,15 +2383,7 @@ int annb_search_multi(annb_index_t *h, const float *queries, int in_space, int64
   ANNB_TRY(multi_enqueue(h, 0, queries, in_space, B, normalize, k, ef_eff, perm, qf, grp, labels_out, dists_out, out_space, 2,
                          nullptr, h->opt_timing != 0, mb, &flagged));
   ANNB_CUDA(cudaStreamSynchronize(h->stream));
-  if (flagged) {
-    int64_t n_over = 0;
-    for (int64_t b = 0; b < B; b++) n_over += mb.hfound[b] < 0;
-    if (n_over) ANNB_TRY(multi_rerun(h, mb, n_over));
-  }
-  for (int64_t b = 0; b < B; b++)
-    if (mb.hfound[b] < k)
-      ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
-  return ANNB_OK;
+  return finish_batch(h, mb, flagged, true);
 }
 
 int annb_search_submit_multi(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
@@ -2502,15 +2417,11 @@ int annb_search_submit_multi(annb_index_t *h, const float *queries, int in_space
   h->stream = lane ? h->stream2 : saved;
   bool flagged = false;
   const int rc = multi_enqueue(h, lane, queries, in_space, B, normalize, k, ef_eff, perm, qf, grp, labels_out, dists_out, out_space,
-                               4 + lane, counters + 64 * lane, false, L.mb, &flagged);
+                               4 + lane, counters + 64 * lane, false, L.batch, &flagged);
   h->stream = saved;
   if (rc != ANNB_OK) return rc;
   L.busy = true;
-  L.B = B;
-  L.k = k;
-  L.hfound = L.mb.hfound;
   L.flagged = flagged;
-  L.multi = true;
   *ticket_out = ticket;
   return ANNB_OK;
 }

@@ -236,6 +236,7 @@ struct Staged {
   float *sd = nullptr;
   int32_t *sfound = nullptr;
   int64_t *sstats = nullptr;
+  float *tables = nullptr;  // the K1 tables of the whole batch once batch_tables has built them
 };
 
 int stage_batch(annb_cellset *cs, const float *queries, int in_space, int64_t B, const int32_t *order, int n_probe, int limit,
@@ -541,6 +542,145 @@ int scan_decision(annb_cellset *cs, int c, const PreparedFilter *f, bool need_ro
   return sync_own_codes(h, &own[(size_t)c]);
 }
 
+// The argument checks of a cell-set search: `bad` = the entry point's own check of B, limit, ef and its pointers,
+// failing with `what`; `pair_limit` = B x n_cells must stay below 2^31 (the per-pair tables of the per-query form)
+int check_search(annb_cellset *cs, bool bad, const char *what, bool pair_limit, int64_t B, const int32_t *order, int in_space,
+                 int n_probe, int limit, int ef) {
+  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  const int C = cs->n_cells;
+  if (bad) ANNB_FAIL(ANNB_EINVAL, "%s", what);
+  if (n_probe < 1 || n_probe > C) ANNB_FAIL(ANNB_EINVAL, "n_probe=%d outside 1..n_cells=%d", n_probe, C);
+  if (!order && !cs->d_centroids) ANNB_FAIL(ANNB_ESTATE, "no centroids: pass the probe order");
+  const int ef_max = std::max(ef, limit);
+  if (ef_max > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, limit)=%d exceeds ANNB_MAX_EF=%d", ef_max, ANNB_MAX_EF);
+  if (pair_limit && (double)B * C >= 2147483647.0) ANNB_FAIL(ANNB_ELIMIT, "B x n_cells=%lld exceeds 2^31-1", (long long)B * C);
+  if (order && in_space != ANNB_DEVICE) ANNB_TRY_RC(check_order(order, B, n_probe, C));
+  return ANNB_OK;
+}
+
+// Every cell's device graph brought up to date, its streams drained and its descriptor read now (buffers move on
+// resize, nothing is cached), then step(c, h) under the same lock: what the search resolves against that snapshot
+template <class Step>
+int sync_cells(annb_cellset *cs, std::vector<GraphDev> &gd, Step step) {
+  ANNB_CUDA(cudaSetDevice(cs->h0->device));
+  gd.resize((size_t)cs->n_cells);
+  for (int c = 0; c < cs->n_cells; c++) {
+    annb_index *h = cs->cells[(size_t)c];
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "cell %d: index not initialised", c);
+    ANNB_TRY_RC(sync_device_graph(h));
+    ANNB_CUDA(cudaStreamSynchronize(h->stream));
+    ANNB_CUDA(cudaStreamSynchronize(h->stream2));
+    gd[(size_t)c] = h->gd;
+    ANNB_TRY_RC(step(c, h));
+  }
+  return ANNB_OK;
+}
+
+// the K1 tables of the whole batch from its normalised queries, built on first use: for the scans, the cells' own
+// launches and the re-runs
+int batch_tables(annb_cellset *cs, Staged &b, int64_t B) {
+  if (b.tables) return ANNB_OK;
+  annb_index *h0 = cs->h0;
+  ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * h0->M * h0->Ks * sizeof(float), (void **)&b.tables));
+  std::lock_guard<std::mutex> lk(h0->mu);
+  return launch_adc_table(h0, b.dq, B, b.tables);
+}
+
+// One launch of cell c on its own handle's stream (after everything queued on the cell set's, which waits for it in
+// turn), with k, mode and selectivity `sel`, its outputs scattered into the cell's rows of the by-cell scratch.  Query
+// rows: every row (rows empty) or `rows`, which read the batch's tables through a query map (gather = false: the
+// bitmap walk's re-run form) or from a gathered copy.  Filter: `filter` for every row, or qf[i] for row i (qf not empty).
+int own_launch(annb_cellset *cs, Staged &b, int64_t B, int limit, int ef, int c, int mode, int k, float sel,
+               const uint32_t *filter, const std::vector<uint32_t> &rows, const std::vector<const uint32_t *> &qf, bool gather) {
+  annb_index *h = cs->cells[(size_t)c];
+  cudaStream_t st = cs->h0->stream;
+  const int TS = cs->h0->M * cs->h0->Ks;
+  const int64_t n = rows.empty() ? B : (int64_t)rows.size();
+  const int64_t out_rows = gather ? n : B;  // through a query map the walk writes row q of its outputs
+  ANNB_TRY_RC(batch_tables(cs, b, B));
+  uint64_t *tl;
+  float *td, *gt = nullptr;
+  int32_t *tf;
+  int64_t *ts = nullptr;
+  uint32_t *dmap = nullptr;
+  const uint32_t **dqf = nullptr;
+  ANNB_TRY_RC(cs_buf(cs, C_TMP_L, (size_t)out_rows * k * 8, (void **)&tl));
+  ANNB_TRY_RC(cs_buf(cs, C_TMP_D, (size_t)out_rows * k * 4, (void **)&td));
+  ANNB_TRY_RC(cs_buf(cs, C_TMP_F, (size_t)out_rows * 4, (void **)&tf));
+  if (b.sstats) ANNB_TRY_RC(cs_buf(cs, C_TMP_S, (size_t)out_rows * 24, (void **)&ts));
+  if (gather) ANNB_TRY_RC(cs_buf(cs, C_GTABLES, (size_t)n * TS * sizeof(float), (void **)&gt));
+  if (!rows.empty()) {
+    ANNB_TRY_RC(cs_buf(cs, C_QMAP, (size_t)n * 4, (void **)&dmap));
+    ANNB_CUDA(cudaMemcpyAsync(dmap, rows.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  }
+  if (!qf.empty()) {
+    ANNB_TRY_RC(cs_buf(cs, C_QF, (size_t)n * sizeof(void *), (void **)&dqf));
+    ANNB_CUDA(cudaMemcpyAsync(dqf, qf.data(), (size_t)n * sizeof(void *), cudaMemcpyHostToDevice, st));
+  }
+  SearchParams p;
+  memset(&p, 0, sizeof(p));
+  p.tables = gather ? gt : b.tables;
+  p.qmap = gather ? nullptr : dmap;
+  p.B = n;
+  p.k = k;
+  p.ef = std::max(ef, k);
+  p.filter = filter;
+  p.query_filter = dqf;
+  p.selectivity = sel;
+  p.out_labels = tl;
+  p.out_dists = td;
+  p.out_found = tf;
+  p.out_stats = ts;
+  std::lock_guard<std::mutex> lk(h->mu);
+  ANNB_CUDA(cudaEventRecord(cs->ev[6], st));
+  ANNB_CUDA(cudaStreamWaitEvent(h->stream, cs->ev[6], 0));
+  if (gather) ANNB_TRY_RC(launch_rows_copy(h, b.tables, gt, dmap, n, TS, false));
+  ANNB_TRY_RC(launch_search(h, p, mode));
+  ANNB_TRY_RC(launch_cell_scatter(h->stream, tl, td, tf, ts, dmap, n, k, cs->n_cells, c, limit, b.sl, b.sd, b.sfound, b.sstats,
+                                  gather));
+  ANNB_CUDA(cudaEventRecord(cs->ev[7], h->stream));
+  ANNB_CUDA(cudaStreamWaitEvent(st, cs->ev[7], 0));
+  return ANNB_OK;
+}
+
+// The last pass of a filtered search over its walked pairs (walked[q * n_cells + c]): `found` read back; the pairs a
+// walk flagged (found = -1) re-run on their cell's bitmap walk, one rerun(c, k, query rows) per (cell, k) with k =
+// pair_k(q, c); `found` read back again if anything ran; then ANNB_EFEWRESULTS where a pair has fewer than its k
+// results, as its cell's own search fails
+template <class PairK, class Rerun>
+int rerun_and_check(annb_cellset *cs, const Staged &b, int64_t B, const std::vector<char> &walked, PairK pair_k, Rerun rerun) {
+  const int C = cs->n_cells;
+  cudaStream_t st = cs->h0->stream;
+  std::vector<int32_t> hfound((size_t)(B * C));
+  ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
+  ANNB_CUDA(cudaStreamSynchronize(st));
+  int64_t reruns = 0;
+  for (int c = 0; c < C; c++) {
+    std::map<int, std::vector<uint32_t>> over;
+    for (int64_t q = 0; q < B; q++)
+      if (walked[(size_t)(q * C + c)] && hfound[(size_t)(q * C + c)] < 0) over[pair_k(q, c)].push_back((uint32_t)q);
+    for (auto &kv : over) {
+      ANNB_TRY_RC(rerun(c, kv.first, kv.second));
+      reruns += (int64_t)kv.second.size();
+    }
+  }
+  cudaEventRecord(cs->ev[3], st);
+  cs->last_rerun_pairs = reruns;
+  if (reruns) {
+    ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
+    ANNB_CUDA(cudaStreamSynchronize(st));
+  }
+  for (int64_t q = 0; q < B; q++)
+    for (int c = 0; c < C; c++) {
+      if (!walked[(size_t)(q * C + c)]) continue;
+      const int k = pair_k(q, c);
+      if (k > 0 && hfound[(size_t)(q * C + c)] < k)
+        ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+    }
+  return ANNB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -606,32 +746,19 @@ int annb_cellset_search(annb_cellset_t *cs, const float *queries, int in_space, 
                         const int32_t *order, int n_probe, int limit, int ef, int flags, uint64_t *labels_out,
                         float *dists_out, int32_t *cells_out, int out_space, uint64_t *part_labels, float *part_dists,
                         int64_t *part_stats) {
-  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  ANNB_TRY_RC(check_search(cs, B < 0 || limit <= 0 || ef <= 0 || !labels_out || !dists_out || !cells_out || (B > 0 && !queries),
+                           "bad B / limit / ef / outputs", false, B, order, in_space, n_probe, limit, ef));
   const int C = cs->n_cells;
-  if (B < 0 || limit <= 0 || ef <= 0 || !labels_out || !dists_out || !cells_out || (B > 0 && !queries))
-    ANNB_FAIL(ANNB_EINVAL, "bad B / limit / ef / outputs");
-  if (n_probe < 1 || n_probe > C) ANNB_FAIL(ANNB_EINVAL, "n_probe=%d outside 1..n_cells=%d", n_probe, C);
-  if (!order && !cs->d_centroids) ANNB_FAIL(ANNB_ESTATE, "no centroids: pass the probe order");
-  if (std::max(ef, limit) > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, limit)=%d exceeds ANNB_MAX_EF=%d", std::max(ef, limit), ANNB_MAX_EF);
-  if (order && in_space != ANNB_DEVICE) ANNB_TRY_RC(check_order(order, B, n_probe, C));
   annb_index *h0 = cs->h0;
-  ANNB_CUDA(cudaSetDevice(h0->device));
-  // every cell's device graph up to date and its descriptor read now: buffers move on resize, nothing is cached
-  std::vector<GraphDev> gd(C);
+  std::vector<GraphDev> gd;
   std::vector<int32_t> kc(C);
   bool fused = !(flags & ANNB_CELLS_GENERIC);
-  for (int c = 0; c < C; c++) {
-    annb_index *h = cs->cells[c];
-    std::lock_guard<std::mutex> lk(h->mu);
-    if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "cell %d: index not initialised", c);
-    ANNB_TRY_RC(sync_device_graph(h));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream2));
-    gd[c] = h->gd;
+  ANNB_TRY_RC(sync_cells(cs, gd, [&](int c, annb_index *h) {
     const int64_t live = h->g.count.load() - h->g.num_deleted;
     kc[c] = (int32_t)std::min<int64_t>(limit, std::max<int64_t>(live, 0));  // container.py:104-105, :119
     fused &= h->g.num_deleted == 0 && !h->opt_force_general && walk4_can_fuse(h) && h->M == 8;
-  }
+    return ANNB_OK;
+  }));
   cs->last_route = fused ? 0 : 1;
   if (B == 0) return ANNB_OK;
   cudaStream_t st = h0->stream;
@@ -681,18 +808,14 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
                                  const int32_t *order, int n_probe, int limit, int ef, int flags, const int *filter_ids,
                                  uint64_t *labels_out, float *dists_out, int32_t *cells_out, int out_space,
                                  uint64_t *part_labels, float *part_dists, int64_t *part_stats) {
-  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  ANNB_TRY_RC(check_search(cs,
+                           B < 0 || limit <= 0 || ef <= 0 || !labels_out || !dists_out || !cells_out || (B > 0 && !queries) ||
+                               !filter_ids,
+                           "bad B / limit / ef / outputs / filter ids", false, B, order, in_space, n_probe, limit, ef));
   const int C = cs->n_cells;
-  if (B < 0 || limit <= 0 || ef <= 0 || !labels_out || !dists_out || !cells_out || (B > 0 && !queries) || !filter_ids)
-    ANNB_FAIL(ANNB_EINVAL, "bad B / limit / ef / outputs / filter ids");
-  if (n_probe < 1 || n_probe > C) ANNB_FAIL(ANNB_EINVAL, "n_probe=%d outside 1..n_cells=%d", n_probe, C);
-  if (!order && !cs->d_centroids) ANNB_FAIL(ANNB_ESTATE, "no centroids: pass the probe order");
   const int ef_max = std::max(ef, limit);
-  if (ef_max > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, limit)=%d exceeds ANNB_MAX_EF=%d", ef_max, ANNB_MAX_EF);
-  if (order && in_space != ANNB_DEVICE) ANNB_TRY_RC(check_order(order, B, n_probe, C));
   annb_index *h0 = cs->h0;
-  ANNB_CUDA(cudaSetDevice(h0->device));
-  std::vector<GraphDev> gd(C);
+  std::vector<GraphDev> gd;
   std::vector<int32_t> kc(C, 0);
   std::vector<const uint32_t *> bits(C, nullptr);
   std::vector<float> sel(C, 0.f);
@@ -700,14 +823,7 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
   std::vector<char> scan(C, 0);  // 1 = the cell's subset is scanned exactly (annb_cellset_set_bruteforce)
   std::vector<const uint8_t *> own_codes(C, nullptr);
   bool fused = !(flags & ANNB_CELLS_GENERIC);
-  for (int c = 0; c < C; c++) {
-    annb_index *h = cs->cells[c];
-    std::lock_guard<std::mutex> lk(h->mu);
-    if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "cell %d: index not initialised", c);
-    ANNB_TRY_RC(sync_device_graph(h));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream2));
-    gd[c] = h->gd;
+  ANNB_TRY_RC(sync_cells(cs, gd, [&](int c, annb_index *h) {
     if (filter_ids[c] != 0) {
       PreparedFilter *f;
       const int rc = find_prepared_filter(h, filter_ids[c], &f);
@@ -727,7 +843,8 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
     }
     int ep, en;
     fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
-  }
+    return ANNB_OK;
+  }));
   // fused route: the cells hnsw_walk4f serves, and N's size (the largest any of them needs alone)
   std::vector<char> own(C, 0);  // 1 = the cell's own filtered launch
   int ep = ef_max <= 64 ? 2 : 4, en = 0, n_own = 0;
@@ -753,8 +870,6 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
   cudaStream_t st = h0->stream;
   Staged b;
   ANNB_TRY_RC(stage_batch(cs, queries, in_space, B, order, n_probe, limit, part_stats != nullptr, b));
-  std::vector<int32_t> hfound;
-  int64_t reruns = 0;
   // the scanned cells: every query that probes one scans its subset with k_c (annb_scan_subset over the whole batch in
   // the per-cell route; the merge reads only the probing queries' rows)
   std::vector<ScanPlan> plans;
@@ -780,14 +895,6 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       }
     ANNB_TRY_RC(check_plans(plans));
   }
-  // the K1 tables of the whole batch, for the scans, the cells' own launches and the re-runs (built once)
-  float *tables = nullptr;
-  auto need_tables = [&]() -> int {
-    if (tables) return ANNB_OK;
-    ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * h0->M * h0->Ks * sizeof(float), (void **)&tables));
-    std::lock_guard<std::mutex> lk(h0->mu);
-    return launch_adc_table(h0, b.dq, B, tables);
-  };
   if (!fused) {
     // one annb_search_prepared per probed cell that is not scanned; a walk with fewer than k_c results fails the call as
     // it fails the cell
@@ -803,8 +910,8 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       for (int r = 0; r < normalize; r++) ANNB_TRY_RC(launch_l2_normalize(h0, b.dq, B, cs->dim));
       StagedScans ss;
       ANNB_TRY_RC(stage_scans(cs, plans, own_codes, gd, true, ss));
-      ANNB_TRY_RC(need_tables());
-      ANNB_TRY_RC(launch_scans(cs, ss, tables, b, limit));
+      ANNB_TRY_RC(batch_tables(cs, b, B));
+      ANNB_TRY_RC(launch_scans(cs, ss, b.tables, b, limit));
       cudaEventRecord(cs->ev[3], st);
     }
   } else {
@@ -824,7 +931,7 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
     ANNB_TRY_RC(host_order(cs, order, in_space, b.dorder, B, n_probe, otmp, &ho));
     StagedScans ss;
     ANNB_TRY_RC(stage_scans(cs, plans, own_codes, gd, false, ss));
-    if (!plans.empty()) ANNB_TRY_RC(need_tables());
+    if (!plans.empty()) ANNB_TRY_RC(batch_tables(cs, b, B));
     cudaEventRecord(cs->ev[2], st);
     if (en > 0) {
       SearchParams p;
@@ -836,85 +943,29 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       if (rc) return rc;
     }
     // the scans, one launch for every scanned cell
-    if (!plans.empty()) ANNB_TRY_RC(launch_scans(cs, ss, tables, b, limit));
-    // one filtered launch of cell c on its own handle's stream (after everything queued on the cell set's, which waits
-    // for it in turn): rows idx (n of them, or every row) of a (B, k_c) output, scattered into the cell's scratch rows
-    auto cell_launch = [&](int c, int mode, const uint32_t *idx, int64_t n) -> int {
-      annb_index *h = cs->cells[c];
-      const int k = kc[c];
-      uint64_t *tl;
-      float *td;
-      int32_t *tf;
-      int64_t *ts = nullptr;
-      ANNB_TRY_RC(cs_buf(cs, C_TMP_L, (size_t)B * k * 8, (void **)&tl));
-      ANNB_TRY_RC(cs_buf(cs, C_TMP_D, (size_t)B * k * 4, (void **)&td));
-      ANNB_TRY_RC(cs_buf(cs, C_TMP_F, (size_t)B * 4, (void **)&tf));
-      if (b.sstats) ANNB_TRY_RC(cs_buf(cs, C_TMP_S, (size_t)B * 24, (void **)&ts));
-      SearchParams p;
-      memset(&p, 0, sizeof(p));
-      p.tables = tables;
-      p.B = idx ? n : B;
-      p.qmap = idx;
-      p.k = k;
-      p.ef = std::max(ef, k);
-      p.filter = bits[c];
-      p.selectivity = sel[c];
-      p.out_labels = tl;
-      p.out_dists = td;
-      p.out_found = tf;
-      p.out_stats = ts;
-      std::lock_guard<std::mutex> lk(h->mu);
-      ANNB_CUDA(cudaEventRecord(cs->ev[6], st));
-      ANNB_CUDA(cudaStreamWaitEvent(h->stream, cs->ev[6], 0));
-      ANNB_TRY_RC(launch_search(h, p, mode));
-      ANNB_TRY_RC(launch_cell_scatter(h->stream, tl, td, tf, ts, idx, p.B, k, C, c, limit, b.sl, b.sd, b.sfound, b.sstats));
-      ANNB_CUDA(cudaEventRecord(cs->ev[7], h->stream));
-      ANNB_CUDA(cudaStreamWaitEvent(st, cs->ev[7], 0));
-      return ANNB_OK;
-    };
+    if (!plans.empty()) ANNB_TRY_RC(launch_scans(cs, ss, b.tables, b, limit));
+    // the cells on their own filtered launch: the whole batch, as the per-cell search walks it
+    const std::vector<uint32_t> every_row;
+    const std::vector<const uint32_t *> no_qf;
     std::vector<char> probed(C, 0);
     for (int64_t i = 0; i < B * n_probe; i++) probed[ho[i]] = 1;
     for (int c = 0; c < C; c++) {
       if (!own[c] || !probed[c]) continue;
-      ANNB_TRY_RC(need_tables());
-      ANNB_TRY_RC(cell_launch(c, 1, nullptr, 0));
+      ANNB_TRY_RC(own_launch(cs, b, B, limit, ef, c, 1, kc[c], sel[c], bits[c], every_row, no_qf, false));
       cs->last_handle_cells++;
     }
-    // (query, cell) pairs a walk flagged (found = -1): re-run on the bitmap walk of that cell, cell by cell
-    hfound.resize((size_t)B * C);
-    ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
-    ANNB_CUDA(cudaStreamSynchronize(st));
-    // (a cell on its own launch walked every query, as the per-cell search does: all its rows count)
-    std::vector<std::vector<uint32_t>> over(C);
+    // the walked pairs (a cell on its own launch walked every query, as the per-cell search does: all its rows count);
+    // flagged ones re-run cell by cell on the batch's tables through a query map
     std::vector<char> walked((size_t)B * C, 0);
     for (int64_t q = 0; q < B; q++) {
       for (int i = 0; i < n_probe; i++) walked[q * C + ho[q * n_probe + i]] = !scan[ho[q * n_probe + i]];
-      for (int c = 0; c < C; c++) {
-        if (own[c] && probed[c]) walked[q * C + c] = 1;
-        if (walked[q * C + c] && hfound[q * C + c] < 0) over[c].push_back((uint32_t)q);
-      }
-    }
-    for (int c = 0; c < C; c++) {
-      if (over[c].empty()) continue;
-      ANNB_TRY_RC(need_tables());
-      uint32_t *dmap;
-      ANNB_TRY_RC(cs_buf(cs, C_QMAP, over[c].size() * 4, (void **)&dmap));
-      ANNB_CUDA(cudaMemcpyAsync(dmap, over[c].data(), over[c].size() * 4, cudaMemcpyHostToDevice, st));
-      ANNB_TRY_RC(cell_launch(c, 2, dmap, (int64_t)over[c].size()));
-      ANNB_CUDA(cudaStreamSynchronize(st));  // the host map is reused by the next cell
-      reruns += (int64_t)over[c].size();
-    }
-    cudaEventRecord(cs->ev[3], st);
-    cs->last_rerun_pairs = reruns;
-    if (reruns) {
-      ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
-      ANNB_CUDA(cudaStreamSynchronize(st));
-    }
-    // a walk with fewer than k_c results: the cell's own search would fail with ANNB_EFEWRESULTS
-    for (int64_t q = 0; q < B; q++)
       for (int c = 0; c < C; c++)
-        if (walked[q * C + c] && kc[c] > 0 && hfound[q * C + c] < kc[c])
-          ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+        if (own[c] && probed[c]) walked[q * C + c] = 1;
+    }
+    ANNB_TRY_RC(rerun_and_check(cs, b, B, walked, [&](int64_t, int c) { return kc[c]; },
+                                [&](int c, int k, const std::vector<uint32_t> &rows) {
+                                  return own_launch(cs, b, B, limit, ef, c, 2, k, sel[c], bits[c], rows, no_qf, false);
+                                }));
   }
   return merge_and_finish(cs, b.sd, b.sl, b.sfound, b.sstats, b.dorder, !order, B, n_probe, limit, labels_out, dists_out, cells_out,
                           out_space, part_labels, part_dists, part_stats);
@@ -934,18 +985,13 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
                               const int32_t *order, int n_probe, int limit, int ef, int flags, const int *query_filter,
                               uint64_t *labels_out, float *dists_out, int32_t *cells_out, int out_space,
                               uint64_t *part_labels, float *part_dists, int64_t *part_stats) {
-  if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
+  ANNB_TRY_RC(check_search(cs,
+                           B < 0 || limit <= 0 || ef <= 0 || !labels_out || !dists_out || !cells_out || (B > 0 && !queries) ||
+                               !query_filter,
+                           "bad B / limit / ef / outputs / filter ids", true, B, order, in_space, n_probe, limit, ef));
   const int C = cs->n_cells;
-  if (B < 0 || limit <= 0 || ef <= 0 || !labels_out || !dists_out || !cells_out || (B > 0 && !queries) || !query_filter)
-    ANNB_FAIL(ANNB_EINVAL, "bad B / limit / ef / outputs / filter ids");
-  if (n_probe < 1 || n_probe > C) ANNB_FAIL(ANNB_EINVAL, "n_probe=%d outside 1..n_cells=%d", n_probe, C);
-  if (!order && !cs->d_centroids) ANNB_FAIL(ANNB_ESTATE, "no centroids: pass the probe order");
   const int ef_max = std::max(ef, limit);
-  if (ef_max > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, limit)=%d exceeds ANNB_MAX_EF=%d", ef_max, ANNB_MAX_EF);
-  if ((double)B * C >= 2147483647.0) ANNB_FAIL(ANNB_ELIMIT, "B x n_cells=%lld exceeds 2^31-1", (long long)B * C);
-  if (order && in_space != ANNB_DEVICE) ANNB_TRY_RC(check_order(order, B, n_probe, C));
   annb_index *h0 = cs->h0;
-  ANNB_CUDA(cudaSetDevice(h0->device));
   // slots: the distinct rows of the id table, each represented by its first query
   std::vector<int32_t> slot((size_t)B);
   std::vector<int64_t> srep;
@@ -960,7 +1006,7 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
   const int64_t S = (int64_t)srep.size();
   auto row_id = [&](int64_t s, int c) { return query_filter[srep[(size_t)s] * C + c]; };
   // every cell's device graph up to date, its filters resolved; per (slot, cell): k, bitmap, selectivity
-  std::vector<GraphDev> gd(C);
+  std::vector<GraphDev> gd;
   std::vector<int64_t> ndel(C);
   std::vector<int32_t> sk((size_t)(S * C), 0);
   std::vector<const uint32_t *> sbits((size_t)(S * C), nullptr);  // nullptr = no filter in this cell
@@ -969,14 +1015,7 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
   std::vector<char> sscan((size_t)(S * C), 0);  // 1 = the pair's subset is scanned exactly (annb_cellset_set_bruteforce)
   std::vector<const uint8_t *> own_codes(C, nullptr);
   bool fused = !(flags & ANNB_CELLS_GENERIC);
-  for (int c = 0; c < C; c++) {
-    annb_index *h = cs->cells[c];
-    std::lock_guard<std::mutex> lk(h->mu);
-    if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "cell %d: index not initialised", c);
-    ANNB_TRY_RC(sync_device_graph(h));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream2));
-    gd[c] = h->gd;
+  ANNB_TRY_RC(sync_cells(cs, gd, [&](int c, annb_index *h) {
     ndel[c] = h->g.num_deleted;
     const int64_t live = std::max<int64_t>(h->g.count.load() - h->g.num_deleted, 0);
     const double nn = (double)std::max<int64_t>(1, h->gd.n);
@@ -1012,7 +1051,8 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
     }
     int ep, en;
     fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
-  }
+    return ANNB_OK;
+  }));
   cs->last_route = fused ? 0 : 1;
   cs->last_rerun_pairs = 0;
   cs->last_handle_cells = 0;
@@ -1059,18 +1099,9 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       else own[i] = 1;
     }
   if (ep == 4 && en > 0) en = en <= 4 ? 4 : (en <= 6 ? 6 : 8);
-  // the K1 tables of the whole batch, for the scans, the own launches and the re-runs (built once)
-  const int TS = h0->M * h0->Ks;
-  float *tables = nullptr;
-  auto need_tables = [&]() -> int {
-    if (tables) return ANNB_OK;
-    ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * TS * sizeof(float), (void **)&tables));
-    std::lock_guard<std::mutex> lk(h0->mu);
-    return launch_adc_table(h0, b.dq, B, tables);
-  };
   StagedScans ss;
   ANNB_TRY_RC(stage_scans(cs, plans, own_codes, gd, !fused, ss));
-  if (!plans.empty()) ANNB_TRY_RC(need_tables());
+  if (!plans.empty()) ANNB_TRY_RC(batch_tables(cs, b, B));
   cudaEventRecord(cs->ev[2], st);
   if (en > 0) {
     // the walk's tables: k per (slot, cell) (0 = skip, own-launch pairs included) and the admission word: the filter's
@@ -1104,55 +1135,8 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
     if (rc) return rc;
   }
   // the scans, after the walk: one launch for all of them (ANNB_CELLS_GENERIC / other geometries: one per cell)
-  if (!plans.empty()) ANNB_TRY_RC(launch_scans(cs, ss, tables, b, limit));
-  // one launch of cell c over query rows `rows` (their tables gathered) with k, on its own handle's stream (after
-  // everything queued on the cell set's, which waits for it in turn); `qf` = each row's bitmap (nullptr = no filter),
-  // or empty for a launch without per-query filters; its outputs scattered into the rows' pairs of the scratch
-  auto rows_launch = [&](int c, int mode, int k, float sel, const std::vector<uint32_t> &rows,
-                         const std::vector<const uint32_t *> &qf) -> int {
-    annb_index *h = cs->cells[c];
-    const int64_t n = (int64_t)rows.size();
-    ANNB_TRY_RC(need_tables());
-    uint64_t *tl;
-    float *td, *gt;
-    int32_t *tf;
-    int64_t *ts = nullptr;
-    uint32_t *dmap;
-    const uint32_t **dqf = nullptr;
-    ANNB_TRY_RC(cs_buf(cs, C_TMP_L, (size_t)n * k * 8, (void **)&tl));
-    ANNB_TRY_RC(cs_buf(cs, C_TMP_D, (size_t)n * k * 4, (void **)&td));
-    ANNB_TRY_RC(cs_buf(cs, C_TMP_F, (size_t)n * 4, (void **)&tf));
-    if (b.sstats) ANNB_TRY_RC(cs_buf(cs, C_TMP_S, (size_t)n * 24, (void **)&ts));
-    ANNB_TRY_RC(cs_buf(cs, C_GTABLES, (size_t)n * TS * sizeof(float), (void **)&gt));
-    ANNB_TRY_RC(cs_buf(cs, C_QMAP, (size_t)n * 4, (void **)&dmap));
-    ANNB_CUDA(cudaMemcpyAsync(dmap, rows.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    if (!qf.empty()) {
-      ANNB_TRY_RC(cs_buf(cs, C_QF, (size_t)n * sizeof(void *), (void **)&dqf));
-      ANNB_CUDA(cudaMemcpyAsync(dqf, qf.data(), (size_t)n * sizeof(void *), cudaMemcpyHostToDevice, st));
-    }
-    SearchParams p;
-    memset(&p, 0, sizeof(p));
-    p.tables = gt;
-    p.B = n;
-    p.k = k;
-    p.ef = std::max(ef, k);
-    p.query_filter = dqf;
-    p.selectivity = sel;
-    p.out_labels = tl;
-    p.out_dists = td;
-    p.out_found = tf;
-    p.out_stats = ts;
-    std::lock_guard<std::mutex> lk(h->mu);
-    ANNB_CUDA(cudaEventRecord(cs->ev[6], st));
-    ANNB_CUDA(cudaStreamWaitEvent(h->stream, cs->ev[6], 0));
-    ANNB_TRY_RC(launch_rows_copy(h, tables, gt, dmap, n, TS, false));
-    ANNB_TRY_RC(launch_search(h, p, mode));
-    ANNB_TRY_RC(launch_cell_scatter(h->stream, tl, td, tf, ts, dmap, n, k, C, c, limit, b.sl, b.sd, b.sfound, b.sstats, true));
-    ANNB_CUDA(cudaEventRecord(cs->ev[7], h->stream));
-    ANNB_CUDA(cudaStreamWaitEvent(st, cs->ev[7], 0));
-    return ANNB_OK;
-  };
-  // own launches, cell by cell: one per (k, kind) -- kind 0 = no filter (annb_search_multi's plain or deletion-aware
+  if (!plans.empty()) ANNB_TRY_RC(launch_scans(cs, ss, b.tables, b, limit));
+  // own launches, cell by cell, over their rows with the rows' tables gathered: one per (k, kind) -- kind 0 = no filter (annb_search_multi's plain or deletion-aware
   // group), 1 = filters hnsw_walk4f takes at that ef, 2 = the others -- as annb_search_multi groups the same rows
   for (int c = 0; c < C; c++) {
     annb_index *h = cs->cells[c];
@@ -1176,41 +1160,17 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       const int k = kv.first.first, kind = kv.first.second;
       int mode = h->opt_force_general == 2 ? 2 : 1;
       if (kind == 0 && ndel[c] == 0 && !h->opt_force_general) mode = 0;
-      ANNB_TRY_RC(rows_launch(c, mode, k, (float)kv.second.s, kv.second.rows, kv.second.qf));
+      ANNB_TRY_RC(own_launch(cs, b, B, limit, ef, c, mode, k, (float)kv.second.s, nullptr, kv.second.rows, kv.second.qf, true));
     }
     if (!groups.empty()) cs->last_handle_cells++;
   }
-  // pairs a walk flagged (found = -1): re-run on the bitmap walk of their cell with their own bitmap, one launch per
-  // (cell, k)
-  std::vector<int32_t> hfound((size_t)(B * C));
-  ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
-  ANNB_CUDA(cudaStreamSynchronize(st));
-  int64_t reruns = 0;
-  for (int c = 0; c < C; c++) {
-    std::map<int, std::pair<std::vector<uint32_t>, std::vector<const uint32_t *>>> over;
-    for (int64_t q = 0; q < B; q++) {
-      if (!walked[(size_t)(q * C + c)] || hfound[(size_t)(q * C + c)] >= 0) continue;
-      const size_t i = (size_t)slot[(size_t)q] * C + c;
-      auto &o = over[sk[i]];
-      o.first.push_back((uint32_t)q);
-      o.second.push_back(sbits[i]);
-    }
-    for (auto &kv : over) {
-      ANNB_TRY_RC(rows_launch(c, 2, kv.first, 1.f, kv.second.first, kv.second.second));
-      reruns += (int64_t)kv.second.first.size();
-    }
-  }
-  cudaEventRecord(cs->ev[3], st);
-  cs->last_rerun_pairs = reruns;
-  if (reruns) {
-    ANNB_CUDA(cudaMemcpyAsync(hfound.data(), b.sfound, hfound.size() * 4, cudaMemcpyDeviceToHost, st));
-    ANNB_CUDA(cudaStreamSynchronize(st));
-  }
-  // a walk with fewer than k results: the cell's own annb_search_multi would fail with ANNB_EFEWRESULTS
-  for (int64_t q = 0; q < B; q++)
-    for (int c = 0; c < C; c++)
-      if (walked[(size_t)(q * C + c)] && hfound[(size_t)(q * C + c)] < sk[(size_t)slot[(size_t)q] * C + c])
-        ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+  // pairs a walk flagged: re-run on the bitmap walk of their cell with their own bitmap, one launch per (cell, k)
+  auto pair_k = [&](int64_t q, int c) { return sk[(size_t)slot[(size_t)q] * C + c]; };
+  ANNB_TRY_RC(rerun_and_check(cs, b, B, walked, pair_k, [&](int c, int k, const std::vector<uint32_t> &rows) {
+    std::vector<const uint32_t *> qf(rows.size());
+    for (size_t j = 0; j < rows.size(); j++) qf[j] = sbits[(size_t)slot[rows[j]] * C + c];
+    return own_launch(cs, b, B, limit, ef, c, 2, k, 1.f, nullptr, rows, qf, true);
+  }));
   return merge_and_finish(cs, b.sd, b.sl, b.sfound, b.sstats, b.dorder, !order, B, n_probe, limit, labels_out, dists_out, cells_out,
                           out_space, part_labels, part_dists, part_stats);
 }

@@ -232,6 +232,22 @@ def test_bruteforce_route_and_forced_reruns(tmp_path):
         got = outcome(lambda: ann.search_numpy(Q, filter=filters, limit=limit))
         assert_same(got, want)
         assert reruns > 0 and e.fallback_queries - before == reruns
+        # the streamed form re-runs the same queries at wait time and returns what the blocking call returns (over the
+        # rows whose filter admits >= limit rows: the streamed form does not shrink the limit)
+        full = [f for f in filters if f not in (few, {'category': {'$eq': 42}})]
+        Qs = Q[:len(full)]
+        qs = idx.prepare_filters(full)
+        try:
+            before = e.fallback_queries
+            blocking = outcome(lambda: idx.search_batch(Qs, limit=limit, filter=qs))
+            blocking_reruns = e.fallback_queries - before
+            assert blocking[0] == 'ok' and blocking_reruns > 0
+            before = e.fallback_queries
+            ticket = idx.search_batch_submit(Qs, limit, filter=qs)
+            assert_same(outcome(lambda: idx.search_batch_wait(ticket)), blocking)
+            assert e.fallback_queries - before == blocking_reruns
+        finally:
+            qs.release()
     finally:
         e.set_option('flagged_en', 0)
 
