@@ -8,6 +8,7 @@
 #include <mutex>
 #include <random>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -372,6 +373,19 @@ int launch_scatter_records(annb_index *h, const uint8_t *d_staged, const uint32_
 // mode: 0 = fast walk (no filter, no deletions), 1 = filtered/deleted walk, kernel chosen automatically
 // (flagged single-list walk when its list fits, else the bitmap walk), 2 = bitmap walk
 int launch_search(annb_index *h, const SearchParams &p, int mode);
+// the work counter of a walk launch and the overflow flag behind it (p.work_counter, or scratch slot 4 when the caller
+// passes none; a caller running several launches concurrently passes its own), zeroed on h->stream
+int walk_counter(annb_index *h, SearchParams &p);
+// f(std::integral_constant<int, EPL>) for the narrowest register list that holds ef entries (32 x EPL, EPL = 2 .. 16)
+template <typename F>
+int with_epl(int ef, F f) {
+  const int epl = (ef + 31) / 32;
+  if (epl <= 2) return f(std::integral_constant<int, 2>());
+  if (epl <= 4) return f(std::integral_constant<int, 4>());
+  if (epl <= 8) return f(std::integral_constant<int, 8>());
+  if (epl <= 16) return f(std::integral_constant<int, 16>());
+  ANNB_FAIL(ANNB_ELIMIT, "ef=%d exceeds ANNB_MAX_EF=%d", ef, ANNB_MAX_EF);
+}
 // code rows wider than ANNB_NARROW_CODE_ROW: links-only device records, the by-id code matrix and hnsw_walk_wide
 inline bool wide_rows(const annb_index *h) { return (size_t)h->M * h->code_bytes > ANNB_NARROW_CODE_ROW; }
 inline int64_t wide_code_stride(const annb_index *h) { return ((int64_t)h->M * h->code_bytes + 15) / 16 * 16; }

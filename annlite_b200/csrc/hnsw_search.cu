@@ -29,20 +29,20 @@
 // Memory layout (DESIGN.md section 3): node record = [maxM0 links][maxM0 neighbour codes], so one
 // hop is one contiguous, coalesced read (384 B for M=8) instead of an adjacency read followed by
 // up to 32 dependent 8-byte gathers.  The per-query table (M*Ks fp32) is staged into shared memory
-// by one TMA bulk copy (cp.async.bulk + mbarrier) per query.
+// by one TMA bulk copy (cp.async.bulk + mbarrier) per query.  Only two-byte codes have a table too big
+// for shared memory (large Ks): hnsw_walk_fast / _chunked / _general then read it from global memory
+// (SMEM_TABLE = false).  One-byte codes are compiled in the shared-memory form only (launch_walk).
 #include <math_constants.h>
 
 #include <algorithm>
 
 #include "annb_internal.h"
 #include "tma_utils.cuh"
-#include "warp_list.cuh"
+#include "walk_common.cuh"
 
 namespace {
 
-constexpr uint32_t EMPTY_LINK = 0xffffffffu;
 constexpr uint32_t EXPANDED_BIT = 0x80000000u;
-constexpr uint32_t ID_MASK = 0x7fffffffu;
 
 // ---- code row in registers -------------------------------------------------------------------
 template <int CR>
@@ -114,24 +114,6 @@ __device__ __forceinline__ void load_table(float *dst, const float *__restrict__
   }
 }
 
-// Next query of the persistent loop: ONE lane bumps the work counter (a predicated instruction, not a branch) and
-// the value is spread with a warp REDUCTION: REDUX delivers it in a uniform register, so ptxas can prove that the
-// loop exit is warp-uniform.  With `__shfl_sync(qi, 0)` it cannot, and then guards every warp-level operation of the
-// loop body with a BRA.DIV convergence check.
-__device__ __forceinline__ int64_t next_query(unsigned int *counter, int lane) {
-  unsigned qi = 0;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.eq.u32 p, %2, 0;\n"
-      "@p atom.global.add.u32 %0, [%1], 1;\n"
-      "}\n"
-      : "+r"(qi)
-      : "l"(counter), "r"(lane)
-      : "memory");
-  return (int64_t)__reduce_max_sync(FULL_MASK, qi);
-}
-
 struct Walk {
   uint32_t node;   // node reached on level 0
   float dist;      // its distance
@@ -195,57 +177,6 @@ __device__ __forceinline__ Walk descend(const GraphDev &g, const float *T, int l
   }
   w.node = rec;
   return w;
-}
-
-template <int EPL>
-__device__ __forceinline__ void write_results(const GraphDev &g, const SearchParams &p, int64_t q, const WarpList<EPL> &L,
-                                              int lane, int hops, int nbrs, int evals) {
-  const int k = p.k;
-  bool tie = false;
-  int found = 0;
-#pragma unroll
-  for (int e = 0; e < EPL; e++) {
-    const int pos = e * 32 + lane;
-    const bool have = L.v[e] != LIST_EMPTY_VAL && pos < k;
-    found += __popc(__ballot_sync(FULL_MASK, have));
-    // tie detection between adjacent list positions
-    float nk = __shfl_down_sync(FULL_MASK, L.k[e], 1);
-    const float first_next = (e + 1 < EPL) ? __shfl_sync(FULL_MASK, L.k[(e + 1 < EPL) ? e + 1 : e], 0) : CUDART_INF_F;
-    if (lane == 31) nk = first_next;
-    tie |= have && (pos + 1 < k) && (nk == L.k[e]);
-    if (pos < k) {
-      p.out_dists[q * k + pos] = have ? L.k[e] : CUDART_INF_F;
-      p.out_labels[q * k + pos] = have ? __ldg(g.labels + (L.v[e] & ID_MASK)) : (uint64_t)UINT64_MAX;
-    }
-  }
-  tie = __any_sync(FULL_MASK, tie);
-  if (tie) {
-    // rows must be ascending by (dist, label) (hnsw_bindings.cpp:346-351); equal distances are
-    // rare, fix them up serially
-    __syncwarp();
-    if (lane == 0) {
-      for (int i = 1; i < found; i++) {
-        float d = p.out_dists[q * k + i];
-        uint64_t l = p.out_labels[q * k + i];
-        int j = i - 1;
-        while (j >= 0 && p.out_dists[q * k + j] == d && p.out_labels[q * k + j] > l) {
-          p.out_dists[q * k + j + 1] = p.out_dists[q * k + j];
-          p.out_labels[q * k + j + 1] = p.out_labels[q * k + j];
-          j--;
-        }
-        p.out_dists[q * k + j + 1] = d;
-        p.out_labels[q * k + j + 1] = l;
-      }
-    }
-  }
-  if (lane == 0) {
-    p.out_found[q] = found;
-    if (p.out_stats) {
-      p.out_stats[q * 3 + 0] = hops;
-      p.out_stats[q * 3 + 1] = nbrs;
-      p.out_stats[q * 3 + 2] = evals;
-    }
-  }
 }
 
 // =================================================================================================
@@ -876,20 +807,7 @@ __global__ void hnsw_walk_flagged(const GraphDev g, const SearchParams p, const 
     }
     if (__any_sync(FULL_MASK, tie)) {
       __syncwarp();
-      if (lane == 0) {
-        for (int i = 1; i < found; i++) {
-          float dd = p.out_dists[q * k + i];
-          uint64_t ll = p.out_labels[q * k + i];
-          int j = i - 1;
-          while (j >= 0 && p.out_dists[q * k + j] == dd && p.out_labels[q * k + j] > ll) {
-            p.out_dists[q * k + j + 1] = p.out_dists[q * k + j];
-            p.out_labels[q * k + j + 1] = p.out_labels[q * k + j];
-            j--;
-          }
-          p.out_dists[q * k + j + 1] = dd;
-          p.out_labels[q * k + j + 1] = ll;
-        }
-      }
+      if (lane == 0) sort_ties(p, q * k, found);
     }
     if (lane == 0) {
       p.out_found[q] = found;
@@ -905,12 +823,6 @@ __global__ void hnsw_walk_flagged(const GraphDev g, const SearchParams p, const 
 // =================================================================================================
 // bitmap path: deletions and/or filter (literal two-structure walk with an exact visited set)
 // =================================================================================================
-__device__ __forceinline__ uint64_t pack_cand(float d, uint32_t id) { return ((uint64_t)__float_as_uint(d) << 32) | id; }
-__device__ __forceinline__ float cand_d(uint64_t c) { return __uint_as_float((uint32_t)(c >> 32)); }
-__device__ __forceinline__ uint32_t cand_id(uint64_t c) { return (uint32_t)c; }
-
-constexpr int SBAG = 256;  // candidate bag entries kept in shared memory per warp (spills to global beyond)
-
 // PQF: as in hnsw_walk_flagged, the bitmap of query row q is p.query_filter[q]
 template <int EPL, int CR, int CB, bool SMEM_TABLE, bool PQF>
 __global__ void hnsw_walk_general(const GraphDev g, const SearchParams p, const int has_del, const int table_stride_bytes) {
@@ -1233,143 +1145,74 @@ LaunchGeom pick_geometry(annb_index *h, size_t table_bytes_in, size_t extra_per_
   return best;
 }
 
-template <int EPL, int CR, int CB, bool PQF>
-int launch_walk(annb_index *h, const SearchParams &p_in, bool general) {
-  SearchParams p = p_in;
-  const size_t table_bytes = (size_t)h->M * h->Ks * sizeof(float);
-  const bool chunked = h->gd.maxM0 > 32;
-  const size_t extra = (size_t)(32 * EPL + (general ? SBAG : (chunked ? 0 : 33))) * sizeof(uint2);
-  int max_warps = 32;
-  LaunchGeom geo = pick_geometry(h, table_bytes, extra, max_warps);
-  int table_stride = geo.smem_table ? (int)((table_bytes + 15) / 16 * 16) : 0;
-  int threads = geo.warps * 32;
-  int has_del = h->g.num_deleted > 0;
-  int occ = geo.ctas_per_sm;
-  bool fits = true;
-  // Large EPL instantiations need > 64 registers/thread: a CTA of 32 warps may not fit the register
-  // file.  ANNB_OCC asks the runtime; on 0 resident CTAs the geometry is re-picked with fewer warps.
-#define ANNB_OCC(KERN)                                                                                                   \
-  do {                                                                                                                   \
-    for (;;) {                                                                                                           \
-      if (geo.smem_bytes > 48 * 1024)                                                                                    \
-        ANNB_CUDA(cudaFuncSetAttribute(KERN, cudaFuncAttributeMaxDynamicSharedMemorySize, geo.smem_bytes));              \
-      int o = 0;                                                                                                         \
-      ANNB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, KERN, threads, geo.smem_bytes));                       \
-      if (o >= 1 || max_warps == 1) {                                                                                    \
-        fits = o >= 1;                                                                                                   \
-        occ = std::max(1, std::min(occ, o));                                                                             \
-        break;                                                                                                           \
-      }                                                                                                                  \
-      max_warps = std::max(1, std::min(max_warps, geo.warps) / 2);                                                       \
-      geo = pick_geometry(h, table_bytes, extra, max_warps);                                                             \
-      table_stride = geo.smem_table ? (int)((table_bytes + 15) / 16 * 16) : 0;                                           \
-      threads = geo.warps * 32;                                                                                          \
-      occ = geo.ctas_per_sm;                                                                                             \
-    }                                                                                                                    \
-    if (!fits) ANNB_FAIL(ANNB_ELIMIT, "kernel does not fit on this device (registers/shared memory)");                   \
-  } while (0)
-  unsigned int *counter = p.work_counter;  // a caller running several launches concurrently passes its own slot
-  int rc;
-  if (!counter) {
-    rc = annb_scratch(h, 4, 256, (void **)&counter);
-    if (rc) return rc;
+// Sets the dynamic shared memory limit of `kern` for `geo` and asks how many of its CTAs fit on an SM.  Large EPL
+// instantiations need > 64 registers/thread, so a CTA of 32 warps may not fit the register file: while none fits, the
+// geometry is re-picked with half the warps.  *occ = resident CTAs per SM (at most geo.ctas_per_sm), 0 = none fits.
+int fit_geometry(annb_index *h, const void *kern, size_t table_bytes, size_t extra, LaunchGeom &geo, int *occ) {
+  for (int max_warps = 32;;) {
+    if (geo.smem_bytes > 48 * 1024) ANNB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, geo.smem_bytes));
+    ANNB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, geo.warps * 32, geo.smem_bytes));
+    if (*occ >= 1 || max_warps == 1) break;
+    max_warps = std::max(1, std::min(max_warps, geo.warps) / 2);
+    geo = pick_geometry(h, table_bytes, extra, max_warps);
   }
-  ANNB_CUDA(cudaMemsetAsync(counter, 0, 8, h->stream));
-  p.work_counter = counter;
-  p.overflow_flag = reinterpret_cast<int32_t *>(counter + 1);
-  if (!general) {
-#define ANNB_LAUNCH_FAST(KERN)                                                                                   \
-  do {                                                                                                           \
-    ANNB_OCC(KERN);                                                                                              \
-    int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * occ, (p.B + geo.warps - 1) / geo.warps);          \
-    KERN<<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, table_stride);                                \
-  } while (0)
-    if (chunked) {
-      if (geo.smem_table) ANNB_LAUNCH_FAST((hnsw_walk_chunked<EPL, CR, CB, true>));
-      else ANNB_LAUNCH_FAST((hnsw_walk_chunked<EPL, CR, CB, false>));
-    } else {
-      if (geo.smem_table) ANNB_LAUNCH_FAST((hnsw_walk_fast<EPL, CR, CB, true>));
-      else ANNB_LAUNCH_FAST((hnsw_walk_fast<EPL, CR, CB, false>));
-    }
-#undef ANNB_LAUNCH_FAST
-  } else {
-    if (geo.smem_table) ANNB_OCC((hnsw_walk_general<EPL, CR, CB, true, PQF>));
-    else ANNB_OCC((hnsw_walk_general<EPL, CR, CB, false, PQF>));
-    int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * occ, (p.B + geo.warps - 1) / geo.warps);
-    int64_t slots = (int64_t)blocks * geo.warps;
-    p.visited_words = (h->gd.n + 31) / 32;
-    // per-warp scratch of the literal walk: visited log and candidate bag.  They start at sizes that cover ordinary
-    // filters and grow (x4, up to the node count: neither can hold more) when a query outgrows them -- a very
-    // selective filter or many deletions make the walk visit a large part of the graph, as the reference's does.
-    const int64_t cap_max = std::max<int64_t>(1 << 15, h->gd.n + 64);
-    int64_t tcap = 1 << 15, ccap = 1 << 14;
-    for (;;) {
-      p.touched_cap = (int)std::min<int64_t>(tcap, cap_max);
-      p.cand_cap = (int)std::min<int64_t>(ccap, cap_max);
-      // keep the per-warp scratch within ~8 GB: fewer resident warps when each needs a lot
-      while (blocks > 1 && (double)blocks * geo.warps * ((double)p.touched_cap * 4 + (double)p.cand_cap * 8) > 8e9) blocks /= 2;
-      slots = (int64_t)blocks * geo.warps;
-      uint32_t *vis;
-      static_assert(sizeof(unsigned int) == 4, "");
-      // scratch slot 5 keeps the visited bitmaps; they are left all-zero by every query, so they are
-      // cleared only when (re)allocated
-      size_t vis_bytes = (size_t)slots * p.visited_words * 4;
-      size_t before = h->scratch_cap[5];
-      if ((rc = annb_scratch(h, 5, vis_bytes, (void **)&vis))) return rc;
-      if (h->scratch_cap[5] != before) ANNB_CUDA(cudaMemsetAsync(vis, 0, h->scratch_cap[5], h->stream));
-      p.visited = vis;
-      if ((rc = annb_scratch(h, 6, (size_t)slots * p.touched_cap * 4, (void **)&p.touched))) return rc;
-      if ((rc = annb_scratch(h, 7, (size_t)slots * p.cand_cap * 8, (void **)&p.cand))) return rc;
-      ANNB_CUDA(cudaMemsetAsync(counter, 0, 8, h->stream));
-      if (geo.smem_table)
-        hnsw_walk_general<EPL, CR, CB, true, PQF><<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, has_del, table_stride);
-      else
-        hnsw_walk_general<EPL, CR, CB, false, PQF><<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, has_del, table_stride);
-      h->launches++;
-      ANNB_CUDA(cudaGetLastError());
-      int32_t flag = 0;
-      ANNB_CUDA(cudaMemcpyAsync(&flag, p.overflow_flag, 4, cudaMemcpyDeviceToHost, h->stream));
-      ANNB_CUDA(cudaStreamSynchronize(h->stream));
-      if (!flag) break;
-      // visited bitmaps may be dirty after an overflow: wipe, then retry with more room
-      ANNB_CUDA(cudaMemsetAsync(h->d_scratch[5], 0, h->scratch_cap[5], h->stream));
-      if (p.touched_cap >= cap_max && p.cand_cap >= cap_max)
-        ANNB_FAIL(ANNB_ELIMIT, "general walk scratch overflow (candidate bag %d / visited log %d entries per query)", p.cand_cap,
-                  p.touched_cap);
-      tcap *= 4;
-      ccap *= 4;
-    }
-    return ANNB_OK;
+  *occ = std::min(*occ, geo.ctas_per_sm);
+  return ANNB_OK;
+}
+
+template <int EPL, int CR, int CB, bool SMEM_TABLE, bool PQF>
+int launch_walk_t(annb_index *h, SearchParams &p, bool general, size_t table_bytes, size_t extra, LaunchGeom geo) {
+  auto fast = h->gd.maxM0 > 32 ? hnsw_walk_chunked<EPL, CR, CB, SMEM_TABLE> : hnsw_walk_fast<EPL, CR, CB, SMEM_TABLE>;
+  auto bitmap = hnsw_walk_general<EPL, CR, CB, SMEM_TABLE, PQF>;
+  int occ;
+  ANNB_TRY_RC(fit_geometry(h, general ? (const void *)bitmap : (const void *)fast, table_bytes, extra, geo, &occ));
+  if (!occ) ANNB_FAIL(ANNB_ELIMIT, "kernel does not fit on this device (registers/shared memory)");
+  const int table_stride = SMEM_TABLE ? (int)((table_bytes + 15) / 16 * 16) : 0;
+  const int threads = geo.warps * 32;
+  const int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * occ, (p.B + geo.warps - 1) / geo.warps);
+  ANNB_TRY_RC(walk_counter(h, p));
+  if (general) {
+    const int has_del = h->g.num_deleted > 0;
+    return run_bitmap_walk(h, p, blocks, geo.warps, "general", [&](int b, const SearchParams &pr) {
+      bitmap<<<b, threads, geo.smem_bytes, h->stream>>>(h->gd, pr, has_del, table_stride);
+    });
   }
-#undef ANNB_OCC
+  fast<<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, table_stride);
   h->launches++;
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;
 }
 
-template <int EPL, int CR, int CB>
-int launch_walk_q(annb_index *h, const SearchParams &p, bool general) {
-  if (general && p.query_filter) return launch_walk<EPL, CR, CB, true>(h, p, general);
-  return launch_walk<EPL, CR, CB, false>(h, p, general);
+template <int EPL, int CR, int CB, bool PQF>
+int launch_walk(annb_index *h, const SearchParams &p_in, bool general) {
+  SearchParams p = p_in;
+  const size_t table_bytes = (size_t)h->M * h->Ks * sizeof(float);
+  const size_t extra = (size_t)(32 * EPL + (general ? SBAG : (h->gd.maxM0 > 32 ? 0 : 33))) * sizeof(uint2);
+  const LaunchGeom geo = pick_geometry(h, table_bytes, extra, 32);
+  if (geo.smem_table) return launch_walk_t<EPL, CR, CB, true, PQF>(h, p, general, table_bytes, extra, geo);
+  // One-byte codes have no global-table form: a row has at most 128 bytes (wider rows take hnsw_walk_wide), so the
+  // table has at most 128 KB and, with at most 6 KB of list and bag, always fits the 227 KB of opt-in shared memory.
+  if constexpr (CB == 1) ANNB_FAIL(ANNB_ESTATE, "internal: a one-byte-code walk table that does not fit in shared memory");
+  else return launch_walk_t<EPL, CR, CB, false, PQF>(h, p, general, table_bytes, extra, geo);
 }
 
-template <int EPL>
-int dispatch_code(annb_index *h, const SearchParams &p, bool general) {
-  const int cr = h->gd.code_row, cb = h->code_bytes;
-  if (cb == 1) {
-    switch (cr) {
-      case 4: return launch_walk_q<EPL, 4, 1>(h, p, general);
-      case 8: return launch_walk_q<EPL, 8, 1>(h, p, general);
-      case 16: return launch_walk_q<EPL, 16, 1>(h, p, general);
-      case 32: return launch_walk_q<EPL, 32, 1>(h, p, general);
-      default: return launch_walk_q<EPL, 0, 1>(h, p, general);
+// f(CR, CB) as std::integral_constant for the index's code rows: CR bytes per row held in registers, 0 = read from memory
+template <typename F>
+int with_code_row(const annb_index *h, F f) {
+  using std::integral_constant;
+  if (h->code_bytes == 1) {
+    switch (h->gd.code_row) {
+      case 4: return f(integral_constant<int, 4>(), integral_constant<int, 1>());
+      case 8: return f(integral_constant<int, 8>(), integral_constant<int, 1>());
+      case 16: return f(integral_constant<int, 16>(), integral_constant<int, 1>());
+      case 32: return f(integral_constant<int, 32>(), integral_constant<int, 1>());
+      default: return f(integral_constant<int, 0>(), integral_constant<int, 1>());
     }
-  } else {
-    switch (cr) {
-      case 8: return launch_walk_q<EPL, 8, 2>(h, p, general);
-      case 16: return launch_walk_q<EPL, 16, 2>(h, p, general);
-      default: return launch_walk_q<EPL, 0, 2>(h, p, general);
-    }
+  }
+  switch (h->gd.code_row) {
+    case 8: return f(integral_constant<int, 8>(), integral_constant<int, 2>());
+    case 16: return f(integral_constant<int, 16>(), integral_constant<int, 2>());
+    default: return f(integral_constant<int, 0>(), integral_constant<int, 2>());
   }
 }
 
@@ -1379,54 +1222,21 @@ int launch_flagged(annb_index *h, const SearchParams &p_in) {
   SearchParams p = p_in;
   const size_t table_bytes = (size_t)h->M * h->Ks * sizeof(float);
   const size_t extra = (size_t)(32 * EPL + 33) * sizeof(uint2);
-  int max_warps = 32;
-  LaunchGeom geo = pick_geometry(h, table_bytes, extra, max_warps);
-  if (!geo.smem_table) return 1;  // not applicable: caller falls back to the bitmap walk
+  // not applicable (1): the caller falls back to the bitmap walk.  smem_table depends on the table size only, so
+  // fit_geometry's smaller geometries keep it.
+  LaunchGeom geo = pick_geometry(h, table_bytes, extra, 32);
+  if (!geo.smem_table) return 1;
   auto kern = p.query_filter ? hnsw_walk_flagged<EPL, CR, CB, true> : hnsw_walk_flagged<EPL, CR, CB, false>;
-  int occ = 0, threads = 0, table_stride = (int)((table_bytes + 15) / 16 * 16);
-  for (;;) {
-    threads = geo.warps * 32;
-    if (geo.smem_bytes > 48 * 1024) ANNB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, geo.smem_bytes));
-    ANNB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, geo.smem_bytes));
-    if (occ >= 1) break;
-    if (max_warps == 1) return 1;
-    max_warps = std::max(1, std::min(max_warps, geo.warps) / 2);
-    geo = pick_geometry(h, table_bytes, extra, max_warps);
-    if (!geo.smem_table) return 1;
-  }
-  occ = std::min(occ, geo.ctas_per_sm);
-  unsigned int *counter = p.work_counter;
-  if (!counter) {
-    int rc = annb_scratch(h, 4, 256, (void **)&counter);
-    if (rc) return rc;
-  }
-  ANNB_CUDA(cudaMemsetAsync(counter, 0, 8, h->stream));
-  p.work_counter = counter;
-  p.overflow_flag = reinterpret_cast<int32_t *>(counter + 1);
+  int occ;
+  ANNB_TRY_RC(fit_geometry(h, (const void *)kern, table_bytes, extra, geo, &occ));
+  if (!occ) return 1;
+  ANNB_TRY_RC(walk_counter(h, p));
   const int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * occ, (p.B + geo.warps - 1) / geo.warps);
-  kern<<<blocks, threads, geo.smem_bytes, h->stream>>>(h->gd, p, h->g.num_deleted > 0 ? 1 : 0, table_stride);
+  kern<<<blocks, geo.warps * 32, geo.smem_bytes, h->stream>>>(h->gd, p, h->g.num_deleted > 0 ? 1 : 0,
+                                                             (int)((table_bytes + 15) / 16 * 16));
   h->launches++;
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;
-}
-
-template <int EPL>
-int dispatch_flagged(annb_index *h, const SearchParams &p) {
-  const int cr = h->gd.code_row, cb = h->code_bytes;
-  if (cb == 1) {
-    switch (cr) {
-      case 4: return launch_flagged<EPL, 4, 1>(h, p);
-      case 8: return launch_flagged<EPL, 8, 1>(h, p);
-      case 16: return launch_flagged<EPL, 16, 1>(h, p);
-      case 32: return launch_flagged<EPL, 32, 1>(h, p);
-      default: return 1;
-    }
-  }
-  switch (cr) {
-    case 8: return launch_flagged<EPL, 8, 2>(h, p);
-    case 16: return launch_flagged<EPL, 16, 2>(h, p);
-    default: return 1;
-  }
 }
 
 }  // namespace
@@ -1450,11 +1260,14 @@ int launch_search(annb_index *h, const SearchParams &p, int mode) {
     for (int e : {2, 4, 8, 16})
       if (epl == 0 && e * 32 >= need && e * 32 >= p.ef) epl = e;
     if (h->opt_flagged_epl > 0 && h->opt_flagged_epl * 32 >= p.ef) epl = (int)h->opt_flagged_epl;
+    auto flagged = [&](auto epl_c) {
+      return with_code_row(h, [&](auto cr, auto cb) {
+        if constexpr (decltype(cr)::value == 0) return 1;  // no register form of the row: not applicable
+        else return launch_flagged<decltype(epl_c)::value, decltype(cr)::value, decltype(cb)::value>(h, p);
+      });
+    };
     int rc = 1;
-    if (epl == 2) rc = dispatch_flagged<2>(h, p);
-    else if (epl == 4) rc = dispatch_flagged<4>(h, p);
-    else if (epl == 8) rc = dispatch_flagged<8>(h, p);
-    else if (epl == 16) rc = dispatch_flagged<16>(h, p);
+    if (epl == 2 || epl == 4 || epl == 8 || epl == 16) rc = with_epl(32 * epl, flagged);
     if (rc != 1) return rc;  // launched (or failed for real); 1 = not applicable -> bitmap walk
   }
   const bool general = mode != 0;
@@ -1463,12 +1276,20 @@ int launch_search(annb_index *h, const SearchParams &p, int mode) {
     if (rc != 1) return rc;
   }
   if (!p.tables) ANNB_FAIL(ANNB_ESTATE, "internal: no tables for the walk");
-  const int epl = (p.ef + 31) / 32;
-  if (epl <= 2) return dispatch_code<2>(h, p, general);
-  if (epl <= 4) return dispatch_code<4>(h, p, general);
-  if (epl <= 8) return dispatch_code<8>(h, p, general);
-  if (epl <= 16) return dispatch_code<16>(h, p, general);
-  ANNB_FAIL(ANNB_ELIMIT, "ef=%d exceeds ANNB_MAX_EF=%d", p.ef, ANNB_MAX_EF);
+  return with_epl(p.ef, [&](auto epl) {
+    return with_code_row(h, [&](auto cr, auto cb) {
+      constexpr int EPL = decltype(epl)::value, CR = decltype(cr)::value, CB = decltype(cb)::value;
+      if (general && p.query_filter) return launch_walk<EPL, CR, CB, true>(h, p, general);
+      return launch_walk<EPL, CR, CB, false>(h, p, general);
+    });
+  });
+}
+
+int walk_counter(annb_index *h, SearchParams &p) {
+  if (!p.work_counter) ANNB_TRY_RC(annb_scratch(h, 4, 256, (void **)&p.work_counter));
+  ANNB_CUDA(cudaMemsetAsync(p.work_counter, 0, 8, h->stream));
+  p.overflow_flag = reinterpret_cast<int32_t *>(p.work_counter + 1);
+  return ANNB_OK;
 }
 
 int launch_pack_rec0(annb_index *h, const uint8_t *d_level0_raw, int64_t n) {

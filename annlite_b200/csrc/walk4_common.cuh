@@ -1,22 +1,19 @@
 // walk4_common.cuh -- pieces shared by hnsw_walk4 (walk_fused.cu) and hnsw_walk4f (walk_flagged4.cu): the
 // order-preserving key image, a level-0 record in registers, the PQ lookup with compile-time M and Ks = 256, the
 // register-resident sorted list (blocked: lane l holds positions l*EPL .. l*EPL+EPL-1) and the in-shared-memory
-// ADC table build (K1 inside the walk).
+// ADC table build (K1 inside the walk), the CTA shape of both kernels and their launch.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "annb_internal.h"
-
-#ifndef FULL_MASK
-#define FULL_MASK 0xffffffffu
-#endif
+#include "walk_common.cuh"
 
 namespace {
 
-constexpr uint32_t EMPTY_LINK = 0xffffffffu;
 constexpr uint32_t EXP_BIT = 0x80000000u;   // list value: node already expanded (empty slots carry it too)
 constexpr uint32_t IDM = 0x7fffffffu;
 constexpr uint32_t KEY_MAX = 0xffffffffu;   // above the image of every finite distance and of +inf
@@ -222,6 +219,57 @@ __device__ __forceinline__ void descend4(const GraphDev &g, const float *T, cons
     // step down: record index on the level below (node id when level == 1)
     rec = __ldg(reinterpret_cast<const uint32_t *>(base + (size_t)rec * g.recu_bytes + g.tail_offu) + 1);
   }
+}
+
+// ---- launch geometry.  Shared memory per query = its table (M KB); the TMA form adds one 8-byte mbarrier per warp.
+// An SM has 228 KB of shared memory and every resident CTA costs 1 KB on top of what it asks for, so at M=8
+// 4 CTAs x 7 warps x 8 KB + 4 KB fills it to the byte: 28 queries per SM in CTAs small enough that the tail of one
+// launch frees SMs piecewise for the next (the two lanes of annb_search_submit overlap that way).  The TMA form
+// (8 bytes more per warp) runs 3 CTAs x 9 warps = 27.  Wider lists need more registers: fewer warps.  hnsw_walk4f
+// (two lists of EP, EN <= 4 or 8 entries; ptxas: 64 registers at EP=2, EN=4, no spills) runs the EPL <= 4 shape.
+constexpr int W4_SMEM_SM = 233472;  // 228 KB per SM
+constexpr int w4_cta_warps(int M, int EPL, bool fused) {
+  return M == 8 ? (EPL <= 4 ? (fused ? 7 : 9) : (EPL == 8 ? 5 : 7)) : 7;
+}
+constexpr int w4_ctas(int M, int EPL, bool fused) {
+  return M == 8 ? (EPL <= 4 ? (fused ? 4 : 3) : (EPL == 8 ? 4 : 2)) : (M == 16 ? 2 : 1);
+}
+constexpr int w4_smem(int M, int EPL, bool fused) { return w4_cta_warps(M, EPL, fused) * (M * 1024 + (fused ? 0 : 8)); }
+constexpr bool w4_fits(int M, int EPL, bool fused) {
+  return w4_ctas(M, EPL, fused) * (w4_smem(M, EPL, fused) + 1024) <= W4_SMEM_SM;
+}
+constexpr int w4_max_threads(int M, int EPL) {
+  return 32 * (w4_cta_warps(M, EPL, true) > w4_cta_warps(M, EPL, false) ? w4_cta_warps(M, EPL, true) : w4_cta_warps(M, EPL, false));
+}
+constexpr int w4_min_ctas(int M, int EPL) {  // register cap = 64K / (max threads x this): must allow either residency
+  const int tf = w4_ctas(M, EPL, true) * w4_cta_warps(M, EPL, true) * 32, tt = w4_ctas(M, EPL, false) * w4_cta_warps(M, EPL, false) * 32;
+  return (tf > tt ? tf : tt) / w4_max_threads(M, EPL);
+}
+
+// One launch of hnsw_walk4 / hnsw_walk4f in the EPL shape: kern(h->gd, p, args...).  The warps_per_cta / ctas_per_sm
+// options cap the shape, and small batches are spread over all SMs instead of filling a few of them.
+template <int M, int EPL, typename Kern, typename... Args>
+int launch_w4(annb_index *h, Kern kern, const SearchParams &p_in, Args... args) {
+  static_assert(w4_fits(M, EPL, true) && w4_fits(M, EPL, false), "walk4 geometry exceeds the SM's shared memory");
+  SearchParams p = p_in;
+  const bool fused = p.queries != nullptr;
+  int warps = w4_cta_warps(M, EPL, fused), ctas = w4_ctas(M, EPL, fused);
+  if (h->opt_warps_per_cta > 0) warps = (int)std::min<int64_t>(h->opt_warps_per_cta, warps);
+  if (h->opt_ctas_per_sm > 0) ctas = (int)std::min<int64_t>(h->opt_ctas_per_sm, ctas);
+  const int64_t per_sm = (p.B + h->sm_count - 1) / h->sm_count;
+  if (per_sm < (int64_t)warps * ctas) {
+    ctas = (int)std::max<int64_t>(1, std::min<int64_t>(ctas, (per_sm + warps - 1) / warps));
+    if (ctas == 1) warps = (int)std::max<int64_t>(1, std::min<int64_t>(warps, per_sm));
+  }
+  const int smem = warps * (M * 1024 + (fused ? 0 : 8));
+  ANNB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 std::max(w4_smem(M, EPL, true), w4_smem(M, EPL, false))));
+  ANNB_TRY_RC(walk_counter(h, p));
+  const int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * ctas, (p.B + warps - 1) / warps);
+  kern<<<blocks, warps * 32, smem, h->stream>>>(h->gd, p, args...);
+  h->launches++;
+  ANNB_CUDA(cudaGetLastError());
+  return ANNB_OK;
 }
 
 

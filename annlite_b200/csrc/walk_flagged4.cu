@@ -49,24 +49,6 @@ namespace {
 
 constexpr uint32_t KEY_FLT_MAX = 0xff7fffffu;  // f2u(FLT_MAX): lowerBound while nothing is admitted (:260)
 
-// Launch geometry = hnsw_walk4's: shared memory per query = its table (M KB, + one mbarrier in the TMA form), 28
-// queries per SM at M = 8 (4 CTAs x 7 warps; TMA form 3 x 9).  Both lists fit the 72 registers that residency allows
-// (ptxas: 64 registers at EP=2, EN=4, no spills in any instantiation).
-constexpr int W4F_SMEM_SM = 233472;  // 228 KB per SM, every resident CTA costs 1 KB on top of what it asks for
-constexpr int w4f_cta_warps(int M, int EP, int EN, bool fused) { return M == 8 ? (fused ? 7 : 9) : 7; }
-constexpr int w4f_ctas(int M, int EP, int EN, bool fused) { return M == 8 ? (fused ? 4 : 3) : (M == 16 ? 2 : 1); }
-constexpr int w4f_smem(int M, int EP, int EN, bool fused) { return w4f_cta_warps(M, EP, EN, fused) * (M * 1024 + (fused ? 0 : 8)); }
-constexpr bool w4f_fits(int M, int EP, int EN, bool fused) {
-  return w4f_ctas(M, EP, EN, fused) * (w4f_smem(M, EP, EN, fused) + 1024) <= W4F_SMEM_SM;
-}
-constexpr int w4f_max_threads(int M, int EP, int EN) {
-  return 32 * (w4f_cta_warps(M, EP, EN, true) > w4f_cta_warps(M, EP, EN, false) ? w4f_cta_warps(M, EP, EN, true) : w4f_cta_warps(M, EP, EN, false));
-}
-constexpr int w4f_min_ctas(int M, int EP, int EN) {  // register cap = 64K / (max threads x this): must allow either residency
-  const int tf = w4f_ctas(M, EP, EN, true) * w4f_cta_warps(M, EP, EN, true) * 32, tt = w4f_ctas(M, EP, EN, false) * w4f_cta_warps(M, EP, EN, false) * 32;
-  return (tf > tt ? tf : tt) / w4f_max_threads(M, EP, EN);
-}
-
 // PQF (per-query filter): query q is admitted by the bitmap p.query_filter[q] (nullptr = "not deleted") instead of the
 // launch's one p.filter; the choice is made at the start of each query.  PQF = false is the single-filter walk.
 //
@@ -83,8 +65,10 @@ constexpr int w4f_min_ctas(int M, int EP, int EN) {  // register cap = 64K / (ma
 // low bits say how to read it: bit 0 = "not deleted" (flip, the query has no filter in this cell: the bitmap is the
 // cell's deletions), bit 1 = the size guard of :270 (the cell has deletions).  Without either bit it is a prepared
 // filter with filter semantics, as in the CELLS form.
+//
+// Launch geometry: hnsw_walk4's EPL <= 4 shape (walk4_common.cuh).
 template <int M, int EP, int EN, bool PQF, bool CELLS>
-__global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP, EN))
+__global__ void __launch_bounds__(w4_max_threads(M, 4), w4_min_ctas(M, 4))
     hnsw_walk4f(const GraphDev g_in, const SearchParams p, const int has_del) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -202,7 +186,7 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       has_slotu = lane < gc.maxM;
     }
     const GraphDev &g = CELLS ? p.cells[__ldg(p.cell_order + q * p.n_probe + ci)] : g_in;
-    // outputs start at entry (CELLS ? oq * p.cell_limit : q * k), written out at each use as in hnsw_walk4
+    // outputs start at entry (CELLS ? oq * p.cell_limit : q * k), computed after the walk as in hnsw_walk4
 
     int hops = 0, nbrs = 0, evals = 1;
     uint32_t cur_uk, rec;
@@ -388,6 +372,7 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       continue;
     }
     // ---- results: the first k admitted entries, ascending (dist, label) (hnsw_bindings.cpp:346-351) ----
+    const int64_t row = CELLS ? oq * p.cell_limit : q * k;
     const int found = min(min(sizeP, ef), k);
     bool tie = false;
     const uint32_t k_next_lane = __shfl_down_sync(FULL_MASK, KP[0], 1);
@@ -396,32 +381,19 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
       const int pos = lane * EP + e;
       if (pos < k) {
         const bool have = pos < found;
-        p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? u2f(KP[e]) : CUDART_INF_F;
-        p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? (p.out_internal ? (uint64_t)(VP[e] & IDM) : __ldg(g.labels + (VP[e] & IDM))) : (uint64_t)UINT64_MAX;
+        p.out_dists[row + pos] = have ? u2f(KP[e]) : CUDART_INF_F;
+        p.out_labels[row + pos] = have ? (p.out_internal ? (uint64_t)(VP[e] & IDM) : __ldg(g.labels + (VP[e] & IDM))) : (uint64_t)UINT64_MAX;
       }
       const uint32_t nk = (e + 1 < EP) ? KP[e + 1 < EP ? e + 1 : e] : k_next_lane;
       tie |= (pos + 1 < found) && (nk == KP[e]) && (e + 1 < EP || lane < 31);
     }
     for (int r = CAPP + lane; r < k; r += 32) {  // k > 32*EP cannot happen (ef >= k, CAPP >= ef); kept for safety
-      p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + r] = CUDART_INF_F;
-      p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + r] = (uint64_t)UINT64_MAX;
+      p.out_dists[row + r] = CUDART_INF_F;
+      p.out_labels[row + r] = (uint64_t)UINT64_MAX;
     }
     if (__any_sync(FULL_MASK, tie)) {
       __syncwarp();
-      if (lane0) {
-        for (int i = 1; i < found; i++) {
-          const float d = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + i];
-          const uint64_t l = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + i];
-          int j = i - 1;
-          while (j >= 0 && p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j] == d && p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j] > l) {
-            p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j];
-            p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j];
-            j--;
-          }
-          p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = d;
-          p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = l;
-        }
-      }
+      if (lane0) sort_ties(p, row, found);
     }
     if (lane0) {
       p.out_found[oq] = found;
@@ -435,55 +407,42 @@ __global__ void __launch_bounds__(w4f_max_threads(M, EP, EN), w4f_min_ctas(M, EP
   }
 }
 
-template <int M, int EP, int EN, bool CELLS = false>
-int launch_walk4f_t(annb_index *h, const SearchParams &p_in) {
-  SearchParams p = p_in;
-  static_assert(w4f_fits(M, EP, EN, true) && w4f_fits(M, EP, EN, false), "walk4f geometry exceeds the SM's shared memory");
+template <int M, int EP, int EN, bool CELLS>
+int launch_walk4f_t(annb_index *h, const SearchParams &p) {
   void (*kern)(const GraphDev, const SearchParams, const int);
   if constexpr (CELLS) kern = p.query_slot ? hnsw_walk4f<M, EP, EN, true, true> : hnsw_walk4f<M, EP, EN, false, true>;
   else kern = p.query_filter ? hnsw_walk4f<M, EP, EN, true, false> : hnsw_walk4f<M, EP, EN, false, false>;
-  const bool fused = p.queries != nullptr;
-  int warps = w4f_cta_warps(M, EP, EN, fused), ctas = w4f_ctas(M, EP, EN, fused);
-  if (h->opt_warps_per_cta > 0) warps = (int)std::min<int64_t>(h->opt_warps_per_cta, warps);
-  if (h->opt_ctas_per_sm > 0) ctas = (int)std::min<int64_t>(h->opt_ctas_per_sm, ctas);
-  const int64_t per_sm = (p.B + h->sm_count - 1) / h->sm_count;
-  if (per_sm < (int64_t)warps * ctas) {
-    ctas = (int)std::max<int64_t>(1, std::min<int64_t>(ctas, (per_sm + warps - 1) / warps));
-    if (ctas == 1) warps = (int)std::max<int64_t>(1, std::min<int64_t>(warps, per_sm));
-  }
-  const int smem = warps * (M * 1024 + (fused ? 0 : 8));
-  ANNB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 std::max(w4f_smem(M, EP, EN, true), w4f_smem(M, EP, EN, false))));
-  unsigned int *counter = p.work_counter;
-  if (!counter) {
-    int rc = annb_scratch(h, 4, 256, (void **)&counter);
-    if (rc) return rc;
-  }
-  ANNB_CUDA(cudaMemsetAsync(counter, 0, 8, h->stream));
-  p.work_counter = counter;
-  p.overflow_flag = reinterpret_cast<int32_t *>(counter + 1);
-  const int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * ctas, (p.B + warps - 1) / warps);
-  kern<<<blocks, warps * 32, smem, h->stream>>>(h->gd, p, h->g.num_deleted > 0 ? 1 : 0);
-  h->launches++;
-  ANNB_CUDA(cudaGetLastError());
-  return ANNB_OK;
+  return launch_w4<M, 4>(h, kern, p, h->g.num_deleted > 0 ? 1 : 0);
 }
 
-template <int M>
-int launch_walk4f_m(annb_index *h, const SearchParams &p, int ep, int en) {
+// f(EP, EN) as std::integral_constant for the instantiated list geometries (walk4f_geometry gives no others); 1 = none
+template <typename F>
+int with_ep_en(int ep, int en, F f) {
+  using std::integral_constant;
   if (ep == 2) {
     switch (en) {
-      case 2: return launch_walk4f_t<M, 2, 2>(h, p);
-      case 3: return launch_walk4f_t<M, 2, 3>(h, p);
-      case 4: return launch_walk4f_t<M, 2, 4>(h, p);
-      case 5: return launch_walk4f_t<M, 2, 5>(h, p);
-      case 6: return launch_walk4f_t<M, 2, 6>(h, p);
-      default: return launch_walk4f_t<M, 2, 8>(h, p);
+      case 2: return f(integral_constant<int, 2>(), integral_constant<int, 2>());
+      case 3: return f(integral_constant<int, 2>(), integral_constant<int, 3>());
+      case 4: return f(integral_constant<int, 2>(), integral_constant<int, 4>());
+      case 5: return f(integral_constant<int, 2>(), integral_constant<int, 5>());
+      case 6: return f(integral_constant<int, 2>(), integral_constant<int, 6>());
+      case 8: return f(integral_constant<int, 2>(), integral_constant<int, 8>());
+    }
+  } else if (ep == 4) {
+    switch (en) {
+      case 4: return f(integral_constant<int, 4>(), integral_constant<int, 4>());
+      case 6: return f(integral_constant<int, 4>(), integral_constant<int, 6>());
+      case 8: return f(integral_constant<int, 4>(), integral_constant<int, 8>());
     }
   }
-  if (en <= 4) return launch_walk4f_t<M, 4, 4>(h, p);
-  if (en <= 6) return launch_walk4f_t<M, 4, 6>(h, p);
-  return launch_walk4f_t<M, 4, 8>(h, p);
+  return 1;
+}
+
+template <int M, bool CELLS>
+int launch_walk4f_m(annb_index *h, const SearchParams &p, int ep, int en) {
+  return with_ep_en(ep, en, [&](auto ep_c, auto en_c) {
+    return launch_walk4f_t<M, decltype(ep_c)::value, decltype(en_c)::value, CELLS>(h, p);
+  });
 }
 
 }  // namespace
@@ -529,9 +488,9 @@ int launch_walk4f(annb_index *h, const SearchParams &p) {
   if (!walk4f_geometry(h, p.ef, (double)p.selectivity, &ep, &en)) return 1;
   if (!p.queries && (!p.tables || (reinterpret_cast<uintptr_t>(p.tables) & 15))) return 1;
   switch (h->M) {
-    case 8: return launch_walk4f_m<8>(h, p, ep, en);
-    case 16: return launch_walk4f_m<16>(h, p, ep, en);
-    case 32: return launch_walk4f_m<32>(h, p, ep, en);
+    case 8: return launch_walk4f_m<8, false>(h, p, ep, en);
+    case 16: return launch_walk4f_m<16, false>(h, p, ep, en);
+    case 32: return launch_walk4f_m<32, false>(h, p, ep, en);
   }
   return 1;
 }
@@ -544,22 +503,5 @@ int launch_walk4f(annb_index *h, const SearchParams &p) {
 int launch_walk4f_cells(annb_index *h, const SearchParams &p, int ep, int en) {
   if (p.B == 0) return ANNB_OK;
   if (!p.queries || h->M != 8 || !p.cell_filter) return 1;
-  if (ep == 2) {
-    switch (en) {
-      case 2: return launch_walk4f_t<8, 2, 2, true>(h, p);
-      case 3: return launch_walk4f_t<8, 2, 3, true>(h, p);
-      case 4: return launch_walk4f_t<8, 2, 4, true>(h, p);
-      case 5: return launch_walk4f_t<8, 2, 5, true>(h, p);
-      case 6: return launch_walk4f_t<8, 2, 6, true>(h, p);
-      case 8: return launch_walk4f_t<8, 2, 8, true>(h, p);
-    }
-    return 1;
-  }
-  if (ep != 4) return 1;
-  switch (en) {
-    case 4: return launch_walk4f_t<8, 4, 4, true>(h, p);
-    case 6: return launch_walk4f_t<8, 4, 6, true>(h, p);
-    case 8: return launch_walk4f_t<8, 4, 8, true>(h, p);
-  }
-  return 1;
+  return launch_walk4f_m<8, true>(h, p, ep, en);
 }

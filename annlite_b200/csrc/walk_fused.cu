@@ -41,30 +41,6 @@
 
 namespace {
 
-// Launch geometry.  Shared memory per query = its table (M KB); the TMA form adds one 8-byte mbarrier per warp.
-// An SM has 228 KB of shared memory and every resident CTA costs 1 KB on top of what it asks for, so at M=8
-// 4 CTAs x 7 warps x 8 KB + 4 KB fills it to the byte: 28 queries per SM in CTAs small enough that the tail of one
-// launch frees SMs piecewise for the next (the two lanes of annb_search_submit overlap that way).  The TMA form
-// (8 bytes more per warp) runs 3 CTAs x 9 warps = 27.  Wider lists need more registers: fewer warps.
-constexpr int W4_SMEM_SM = 233472;  // 228 KB per SM
-constexpr int w4_cta_warps(int M, int EPL, bool fused) {
-  return M == 8 ? (EPL <= 4 ? (fused ? 7 : 9) : (EPL == 8 ? 5 : 7)) : 7;
-}
-constexpr int w4_ctas(int M, int EPL, bool fused) {
-  return M == 8 ? (EPL <= 4 ? (fused ? 4 : 3) : (EPL == 8 ? 4 : 2)) : (M == 16 ? 2 : 1);
-}
-constexpr int w4_smem(int M, int EPL, bool fused) { return w4_cta_warps(M, EPL, fused) * (M * 1024 + (fused ? 0 : 8)); }
-constexpr bool w4_fits(int M, int EPL, bool fused) {
-  return w4_ctas(M, EPL, fused) * (w4_smem(M, EPL, fused) + 1024) <= W4_SMEM_SM;
-}
-constexpr int w4_max_threads(int M, int EPL) {
-  return 32 * (w4_cta_warps(M, EPL, true) > w4_cta_warps(M, EPL, false) ? w4_cta_warps(M, EPL, true) : w4_cta_warps(M, EPL, false));
-}
-constexpr int w4_min_ctas(int M, int EPL) {  // register cap = 64K / (max threads x this): must allow either residency
-  const int tf = w4_ctas(M, EPL, true) * w4_cta_warps(M, EPL, true) * 32, tt = w4_ctas(M, EPL, false) * w4_cta_warps(M, EPL, false) * 32;
-  return (tf > tt ? tf : tt) / w4_max_threads(M, EPL);
-}
-
 // =====================================================================================================
 // CELLS: the multi-cell (IVF) walk of annb_cellset_search.  The work item is a query: its table is built once and then
 // walked over each of its probed cells in probe order (p.cells, p.cell_order; the cells share one PQ codebook), the
@@ -165,8 +141,8 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
       has_slotu = lane < gc.maxM;
     }
     const GraphDev &g = CELLS ? p.cells[__ldg(p.cell_order + q * p.n_probe + ci)] : g_in;
-    // outputs start at entry (CELLS ? oq * p.cell_limit : q * k), written out at each use: a hoisted copy reschedules the
-    // single-graph walk
+    // outputs start at entry (CELLS ? oq * p.cell_limit : q * k), written out at each use until the walk is done: a
+    // copy hoisted above it reschedules the single-graph walk
 
     // ---- greedy descent maxlevel..1 (hnswalg.h:1245-1274), walk4_common.cuh ----
     int hops = 0, nbrs = 0, evals = 1;
@@ -320,6 +296,7 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
     }
 
     // ---- results: the first k list entries, ascending (dist, label) (hnsw_bindings.cpp:346-351) ----
+    const int64_t row = CELLS ? oq * p.cell_limit : q * k;
     const int found = min(size, k);
     bool tie = false;
     const uint32_t k_next_lane = __shfl_down_sync(FULL_MASK, K[0], 1);
@@ -328,29 +305,15 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
       const int pos = lane * EPL + e;
       if (pos < k) {
         const bool have = pos < size;
-        p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? u2f(K[e]) : CUDART_INF_F;
-        p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + pos] = have ? (p.out_internal ? (uint64_t)(V[e] & IDM) : __ldg(g.labels + (V[e] & IDM))) : (uint64_t)UINT64_MAX;
+        p.out_dists[row + pos] = have ? u2f(K[e]) : CUDART_INF_F;
+        p.out_labels[row + pos] = have ? (p.out_internal ? (uint64_t)(V[e] & IDM) : __ldg(g.labels + (V[e] & IDM))) : (uint64_t)UINT64_MAX;
       }
       const uint32_t nk = (e + 1 < EPL) ? K[e + 1 < EPL ? e + 1 : e] : k_next_lane;
       tie |= (pos + 1 < found) && (nk == K[e]) && (e + 1 < EPL || lane < 31);
     }
     if (__any_sync(FULL_MASK, tie)) {
-      // rows must be ascending by (dist, label); equal distances are rare, fix them up serially
       __syncwarp();
-      if (lane0) {
-        for (int i = 1; i < found; i++) {
-          const float d = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + i];
-          const uint64_t l = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + i];
-          int j = i - 1;
-          while (j >= 0 && p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j] == d && p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j] > l) {
-            p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j];
-            p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j];
-            j--;
-          }
-          p.out_dists[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = d;
-          p.out_labels[(CELLS ? oq * p.cell_limit : q * k) + j + 1] = l;
-        }
-      }
+      if (lane0) sort_ties(p, row, found);
     }
     if (lane0) {
       p.out_found[oq] = found;
@@ -364,47 +327,12 @@ __global__ void __launch_bounds__(w4_max_threads(M, EPL), w4_min_ctas(M, EPL)) h
   }
 }
 
-template <int M, int EPL, bool CELLS>
-int launch_walk4_t(annb_index *h, const SearchParams &p_in) {
-  SearchParams p = p_in;
-  static_assert(w4_fits(M, EPL, true) && w4_fits(M, EPL, false), "walk4 geometry exceeds the SM's shared memory");
-  auto kern = hnsw_walk4<M, EPL, CELLS>;
-  const bool fused = p.queries != nullptr;
-  int warps = fused ? w4_cta_warps(M, EPL, true) : w4_cta_warps(M, EPL, false);
-  int ctas = fused ? w4_ctas(M, EPL, true) : w4_ctas(M, EPL, false);
-  if (h->opt_warps_per_cta > 0) warps = (int)std::min<int64_t>(h->opt_warps_per_cta, warps);
-  if (h->opt_ctas_per_sm > 0) ctas = (int)std::min<int64_t>(h->opt_ctas_per_sm, ctas);
-  // small batches: spread the queries over all SMs instead of filling a few of them
-  const int64_t per_sm = (p.B + h->sm_count - 1) / h->sm_count;
-  if (per_sm < (int64_t)warps * ctas) {
-    ctas = (int)std::max<int64_t>(1, std::min<int64_t>(ctas, (per_sm + warps - 1) / warps));
-    if (ctas == 1) warps = (int)std::max<int64_t>(1, std::min<int64_t>(warps, per_sm));
-  }
-  const int smem = warps * (M * 1024 + (fused ? 0 : 8));
-  ANNB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 std::max(w4_smem(M, EPL, true), w4_smem(M, EPL, false))));
-  unsigned int *counter = p.work_counter;
-  if (!counter) {
-    int rc = annb_scratch(h, 4, 256, (void **)&counter);
-    if (rc) return rc;
-  }
-  ANNB_CUDA(cudaMemsetAsync(counter, 0, 8, h->stream));
-  p.work_counter = counter;
-  p.overflow_flag = reinterpret_cast<int32_t *>(counter + 1);
-  const int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * ctas, (p.B + warps - 1) / warps);
-  kern<<<blocks, warps * 32, smem, h->stream>>>(h->gd, p);
-  h->launches++;
-  ANNB_CUDA(cudaGetLastError());
-  return ANNB_OK;
-}
-
 template <int M, bool CELLS>
-int launch_walk4_m(annb_index *h, const SearchParams &p) {
-  const int epl = (p.ef + 31) / 32;
-  if (epl <= 2) return launch_walk4_t<M, 2, CELLS>(h, p);
-  if (epl <= 4) return launch_walk4_t<M, 4, CELLS>(h, p);
-  if (epl <= 8) return launch_walk4_t<M, 8, CELLS>(h, p);
-  return launch_walk4_t<M, 16, CELLS>(h, p);
+int launch_walk4_m(annb_index *h, const SearchParams &p, int ef) {
+  return with_epl(ef, [&](auto epl) {  // the callers hold ef to ANNB_MAX_EF
+    constexpr int EPL = decltype(epl)::value;
+    return launch_w4<M, EPL>(h, hnsw_walk4<M, EPL, CELLS>, p);
+  });
 }
 
 }  // namespace
@@ -435,9 +363,9 @@ int launch_walk4(annb_index *h, const SearchParams &p) {
   if (!p.queries && (reinterpret_cast<uintptr_t>(p.tables) & 15)) return 1;  // TMA needs 16-byte alignment
   if (p.ef > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "ef=%d exceeds ANNB_MAX_EF=%d", p.ef, ANNB_MAX_EF);
   switch (h->M) {
-    case 8: return launch_walk4_m<8, false>(h, p);
-    case 16: return launch_walk4_m<16, false>(h, p);
-    case 32: return launch_walk4_m<32, false>(h, p);
+    case 8: return launch_walk4_m<8, false>(h, p, p.ef);
+    case 16: return launch_walk4_m<16, false>(h, p, p.ef);
+    case 32: return launch_walk4_m<32, false>(h, p, p.ef);
   }
   return 1;
 }
@@ -450,9 +378,5 @@ int launch_walk4_cells(annb_index *h, const SearchParams &p) {
   if (!p.queries || h->M != 8) return 1;
   const int ef_max = std::max(p.ef, p.cell_limit);  // the largest max(ef, k_c) of any cell sizes the list
   if (ef_max > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, limit)=%d exceeds ANNB_MAX_EF=%d", ef_max, ANNB_MAX_EF);
-  const int epl = (ef_max + 31) / 32;
-  if (epl <= 2) return launch_walk4_t<8, 2, true>(h, p);
-  if (epl <= 4) return launch_walk4_t<8, 4, true>(h, p);
-  if (epl <= 8) return launch_walk4_t<8, 8, true>(h, p);
-  return launch_walk4_t<8, 16, true>(h, p);
+  return launch_walk4_m<8, true>(h, p, ef_max);
 }

@@ -22,33 +22,11 @@
 #include <algorithm>
 
 #include "annb_internal.h"
-#include "warp_list.cuh"
+#include "walk_common.cuh"
 
 namespace {
 
-constexpr uint32_t EMPTY_LINK = 0xffffffffu;
-constexpr uint32_t ID_MASK = 0x7fffffffu;
-constexpr int SBAG = 256;  // candidate bag entries kept in shared memory per warp (spills to global beyond)
 constexpr int WIDE_WARPS = 8;
-
-// next query of the persistent loop (hnsw_search.cu: next_query, same reasoning: REDUX keeps the exit warp-uniform)
-__device__ __forceinline__ int64_t next_query(unsigned int *counter, int lane) {
-  unsigned qi = 0;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.eq.u32 p, %2, 0;\n"
-      "@p atom.global.add.u32 %0, [%1], 1;\n"
-      "}\n"
-      : "+r"(qi)
-      : "l"(counter), "r"(lane)
-      : "memory");
-  return (int64_t)__reduce_max_sync(FULL_MASK, qi);
-}
-
-__device__ __forceinline__ uint64_t pack_cand(float d, uint32_t id) { return ((uint64_t)__float_as_uint(d) << 32) | id; }
-__device__ __forceinline__ float cand_d(uint64_t c) { return __uint_as_float((uint32_t)(c >> 32)); }
-__device__ __forceinline__ uint32_t cand_id(uint64_t c) { return (uint32_t)c; }
 
 // what one distance needs: the query (or the query's table) and the codebook
 struct Scorer {
@@ -94,56 +72,6 @@ __device__ __forceinline__ float score_row(const Scorer &s, const uint8_t *row) 
     }
   }
   return r;
-}
-
-// hnsw_search.cu: write_results, unchanged
-template <int EPL>
-__device__ __forceinline__ void write_results(const GraphDev &g, const SearchParams &p, int64_t q, const WarpList<EPL> &L,
-                                              int lane, int hops, int nbrs, int evals) {
-  const int k = p.k;
-  bool tie = false;
-  int found = 0;
-#pragma unroll
-  for (int e = 0; e < EPL; e++) {
-    const int pos = e * 32 + lane;
-    const bool have = L.v[e] != LIST_EMPTY_VAL && pos < k;
-    found += __popc(__ballot_sync(FULL_MASK, have));
-    float nk = __shfl_down_sync(FULL_MASK, L.k[e], 1);
-    const float first_next = (e + 1 < EPL) ? __shfl_sync(FULL_MASK, L.k[(e + 1 < EPL) ? e + 1 : e], 0) : CUDART_INF_F;
-    if (lane == 31) nk = first_next;
-    tie |= have && (pos + 1 < k) && (nk == L.k[e]);
-    if (pos < k) {
-      p.out_dists[q * k + pos] = have ? L.k[e] : CUDART_INF_F;
-      p.out_labels[q * k + pos] = have ? __ldg(g.labels + (L.v[e] & ID_MASK)) : (uint64_t)UINT64_MAX;
-    }
-  }
-  tie = __any_sync(FULL_MASK, tie);
-  if (tie) {
-    // rows ascending by (dist, label) (hnsw_bindings.cpp:346-351)
-    __syncwarp();
-    if (lane == 0) {
-      for (int i = 1; i < found; i++) {
-        float d = p.out_dists[q * k + i];
-        uint64_t l = p.out_labels[q * k + i];
-        int j = i - 1;
-        while (j >= 0 && p.out_dists[q * k + j] == d && p.out_labels[q * k + j] > l) {
-          p.out_dists[q * k + j + 1] = p.out_dists[q * k + j];
-          p.out_labels[q * k + j + 1] = p.out_labels[q * k + j];
-          j--;
-        }
-        p.out_dists[q * k + j + 1] = d;
-        p.out_labels[q * k + j + 1] = l;
-      }
-    }
-  }
-  if (lane == 0) {
-    p.out_found[q] = found;
-    if (p.out_stats) {
-      p.out_stats[q * 3 + 0] = hops;
-      p.out_stats[q * 3 + 1] = nbrs;
-      p.out_stats[q * 3 + 2] = evals;
-    }
-  }
 }
 
 // PQF: the bitmap of query row q is p.query_filter[q] (nullptr = "not deleted"); q_smem: the query is staged in
@@ -458,46 +386,12 @@ int launch_wide_t(annb_index *h, const SearchParams &p_in) {
   int occ = 0;
   ANNB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
   if (occ < 1) ANNB_FAIL(ANNB_ELIMIT, "hnsw_walk_wide does not fit on this device (registers/shared memory)");
-  unsigned int *counter = p.work_counter;
-  int rc;
-  if (!counter && (rc = annb_scratch(h, 4, 256, (void **)&counter))) return rc;
-  p.work_counter = counter;
-  p.overflow_flag = reinterpret_cast<int32_t *>(counter + 1);
-  int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * occ, (p.B + warps - 1) / warps);
-  p.visited_words = (h->gd.n + 31) / 32;
-  // per-warp scratch as for hnsw_walk_general (hnsw_search.cu: launch_walk): visited log and candidate bag start at
-  // sizes that cover ordinary searches and grow x4, up to the node count, when a query outgrows them
-  const int64_t cap_max = std::max<int64_t>(1 << 15, h->gd.n + 64);
-  int64_t tcap = 1 << 15, ccap = 1 << 14;
-  for (;;) {
-    p.touched_cap = (int)std::min<int64_t>(tcap, cap_max);
-    p.cand_cap = (int)std::min<int64_t>(ccap, cap_max);
-    while (blocks > 1 && (double)blocks * warps * ((double)p.touched_cap * 4 + (double)p.cand_cap * 8) > 8e9) blocks /= 2;
-    const int64_t slots = (int64_t)blocks * warps;
-    uint32_t *vis;
-    // scratch slot 5 keeps the visited bitmaps; every query leaves them all-zero, so they are cleared on (re)allocation
-    const size_t before = h->scratch_cap[5];
-    if ((rc = annb_scratch(h, 5, (size_t)slots * p.visited_words * 4, (void **)&vis))) return rc;
-    if (h->scratch_cap[5] != before) ANNB_CUDA(cudaMemsetAsync(vis, 0, h->scratch_cap[5], h->stream));
-    p.visited = vis;
-    if ((rc = annb_scratch(h, 6, (size_t)slots * p.touched_cap * 4, (void **)&p.touched))) return rc;
-    if ((rc = annb_scratch(h, 7, (size_t)slots * p.cand_cap * 8, (void **)&p.cand))) return rc;
-    ANNB_CUDA(cudaMemsetAsync(counter, 0, 8, h->stream));
-    kern<<<blocks, threads, smem, h->stream>>>(h->gd, p, wd, h->g.num_deleted > 0 ? 1 : 0, q_smem);
-    h->launches++;
-    ANNB_CUDA(cudaGetLastError());
-    int32_t flag = 0;
-    ANNB_CUDA(cudaMemcpyAsync(&flag, p.overflow_flag, 4, cudaMemcpyDeviceToHost, h->stream));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream));
-    if (!flag) break;
-    // visited bitmaps may be dirty after an overflow: wipe, then retry with more room
-    ANNB_CUDA(cudaMemsetAsync(h->d_scratch[5], 0, h->scratch_cap[5], h->stream));
-    if (p.touched_cap >= cap_max && p.cand_cap >= cap_max)
-      ANNB_FAIL(ANNB_ELIMIT, "wide walk scratch overflow (candidate bag %d / visited log %d entries per query)", p.cand_cap, p.touched_cap);
-    tcap *= 4;
-    ccap *= 4;
-  }
-  return ANNB_OK;
+  ANNB_TRY_RC(walk_counter(h, p));
+  const int blocks = (int)std::min<int64_t>((int64_t)h->sm_count * occ, (p.B + warps - 1) / warps);
+  const int has_del = h->g.num_deleted > 0 ? 1 : 0;
+  return run_bitmap_walk(h, p, blocks, warps, "wide", [&](int b, const SearchParams &pr) {
+    kern<<<b, threads, smem, h->stream>>>(h->gd, pr, wd, has_del, q_smem);
+  });
 }
 
 template <int EPL>
@@ -512,10 +406,5 @@ int launch_wide_e(annb_index *h, const SearchParams &p) {
 int launch_walk_wide(annb_index *h, const SearchParams &p) {
   if (p.B == 0) return ANNB_OK;
   if (!h->d_wide_codes || h->gd.n == 0) ANNB_FAIL(ANNB_ESTATE, "internal: the wide device graph is not built");
-  const int epl = (p.ef + 31) / 32;
-  if (epl <= 2) return launch_wide_e<2>(h, p);
-  if (epl <= 4) return launch_wide_e<4>(h, p);
-  if (epl <= 8) return launch_wide_e<8>(h, p);
-  if (epl <= 16) return launch_wide_e<16>(h, p);
-  ANNB_FAIL(ANNB_ELIMIT, "ef=%d exceeds ANNB_MAX_EF=%d", p.ef, ANNB_MAX_EF);
+  return with_epl(p.ef, [&](auto epl) { return launch_wide_e<decltype(epl)::value>(h, p); });
 }

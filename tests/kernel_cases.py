@@ -5,11 +5,10 @@ bool template arguments as plain integers (`(int)16` -> 16, `(bool)1` / `true` -
 (`unsigned char` -> u8).  `library_keys()` reads them from the built library (cuobjdump -symbols | cu++filt), and
 `test_gpu_instances.captured_keys` reduces the kernel names the CUDA profiler records with the same `kernel_key`.
 
-Each key is in exactly one of three groups:
+Each key is in exactly one of two groups:
   COVERED      keys that some GPU case of tests/test_gpu_instances.py (CASES below) asserts it launched;
-  UNREACHABLE  key -> why no input reaches it;
   ELSEWHERE    key -> the existing test that runs it (kernels off the search and scan paths).
-tests/test_kernel_inventory.py asserts that the three groups partition the library's keys exactly."""
+tests/test_kernel_inventory.py asserts that the two groups partition the library's keys exactly."""
 import os
 import re
 import shutil
@@ -264,17 +263,6 @@ for G in (1, 2, 3, 8):
     _case(f'merge-G{G}', 'merge', None, {}, [], ['merge_sorted_kernel'], G=G)
 
 COVERED = set().union(*(c['keys'] for c in CASES))
-
-# ---- keys no input reaches -------------------------------------------------------------------------------------------
-_NO_GLOBAL_U8 = ('one-byte codes: a code row of at most 128 bytes (wider rows take hnsw_walk_wide) has a table of at most '
-                 '128 KB, which always fits shared memory (pick_geometry), so the launchers never pick smem_table=false')
-UNREACHABLE = {}
-for epl in EPLS:
-    for cr in (4, 8, 16, 32, 0):
-        UNREACHABLE[f'hnsw_walk_fast<{epl},{cr},1,0>'] = _NO_GLOBAL_U8
-        UNREACHABLE[f'hnsw_walk_chunked<{epl},{cr},1,0>'] = _NO_GLOBAL_U8
-        for pqf in (0, 1):
-            UNREACHABLE[f'hnsw_walk_general<{epl},{cr},1,0,{pqf}>'] = _NO_GLOBAL_U8
 
 # ---- kernels of other paths and the tests that run them -------------------------------------------------------------
 ELSEWHERE = {
