@@ -7,7 +7,10 @@
 //   * the new node x links to the M_ nearest of its ef_construction candidates, farthest first;
 //   * a selected neighbour r with room appends x; a full one keeps x and those of its neighbours that are NOT
 //     closer to x than r itself is (in descending id order, at most maxM0 of them).
-// hnsw_build.cpp restates that on the host, byte for byte.  Here the same rules run batch-wise on the device:
+// hnsw_build.cpp restates that on the host, byte for byte.  Here the same rules run batch-wise on the device, with one
+// difference of storage order: a rewritten list is stored here in descending id, while the reference's queue gives
+// its entries (all of key d(x, r)) back in the pop order of an equal-key heap.  The set of links is the same; the
+// order is kept so that a build, and every search over it, stays what earlier versions of this builder made.
 //
 //   phase 1 (host, existing code)  every node that owns upper-level lists (~1/M of the rows, levels drawn first with
 //            the index's own generator) plus a few thousand level-0 rows are inserted by hnsw_insert_rows: the whole
@@ -25,9 +28,11 @@
 // concurrent insertions see a partially linked graph); batches grow with the graph (<= 1/16 of it by default, <= 65536 rows).
 // The result is deterministic: phase 1 inserts on one host thread and phase 2 fixes the order of every write, so the
 // same rows give the same graph on every run and machine, whatever num_threads is.
-// The graph is NOT the one a sequential build makes; what is checked is what matters for the path: every structural
-// invariant (HostGraph::validate), oracle parity of searches over the result, and recall against a host-built
-// graph of the same data (tests/test_gpu_build.py).
+// The graph is NOT the one a sequential build makes, but every rule above is exact: tests/test_gpu_build_model.py
+// compares the result byte for byte with a restatement of phase 2, which reproduces the sequential host build when
+// its batches are one row and rewritten lists keep the reference's order (tests/test_build_model.py);
+// tests/test_gpu_build.py checks the structural invariants, search parity over the result and recall against a
+// host-built graph.
 //
 // gpu_build_cells runs the same build for the shares of a cell-set insertion together (annb_cellset_add_items):
 // phase 1 on a host thread per cell, phase 2 in rounds where every cell inserts its next batch with one multi-cell walk

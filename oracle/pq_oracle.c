@@ -18,8 +18,8 @@
  *
  * Every function cites the reference file:line it follows (paths relative to /root/reference).
  *
- * The last two functions of the file (orc_single_list_walk, orc_flagged_walk) are the exception and
- * are marked as such: scalar models of the PRODUCT's walks, run beside the restatement by CPU tests.
+ * The functions from orc_single_list_walk on are the exception and are marked as such: scalar models of
+ * the PRODUCT's walks and of its batched GPU build's back-links, run beside the restatement by tests.
  */
 #include <float.h>
 #include <math.h>
@@ -715,4 +715,92 @@ ORC_API int orc_two_list_walk(const uint8_t *level0, uint64_t size_per_elem, uin
   }
   free(P); free(N); free(res);
   return 0;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* NOT the reference: one batch of back-links of the product's batched GPU build             */
+/* ------------------------------------------------------------------------------------------ */
+
+/* The back-link step of oracle/gpu_build_model.py (whose numpy form, backlinks_numpy, is this function's
+ * CPU-side reference).  Rows i = 0..B-1 of a batch became nodes x = first + i; row i links back to its
+ * min(found[i], k) candidates r = sel[i*k + j] at distance dist[i*k + j], in pair order p = i*k + j.  A
+ * neighbour with room appends x; a full one becomes [x] + those of its neighbours c with !(D(x, c) < d),
+ * in descending id, at most maxM0 in all: hnswalg.h:575-616 in PQ mode (hnsw_build.cpp connect()), where
+ * D(x, c) = PQLookup of c's code in x's table.  queue_order = 0 stores that list in descending id, as the
+ * GPU builder does; 1 stores it in the order the reference's queue gives it back: every kept entry has the
+ * same key d, so that is the pop order of a max-heap of equal keys pushed in descending id (heap_pop_order).
+ * Slots past a rewritten list's count keep their old bytes, as the host builder leaves them.  level0: host-layout records (count u16 at 0, links u32 from byte 4,
+ * u8 codes at offset_data).  counts[0..2] += appends, rewrites, rewrites that dropped a neighbour. */
+/* The order in which std::priority_queue (libstdc++ std::pop_heap / __adjust_heap) gives back n entries of
+ * EQUAL key pushed as 0..n-1: push_heap moves nothing, and each pop takes the front and sifts the last entry in
+ * along the right children.  out[s] = the push position of the s-th entry popped. */
+static void heap_pop_order(int n, int *out) {
+  int a[2048];
+  for (int i = 0; i < n; i++) a[i] = i;
+  for (int s = 0, len = n; len > 0; s++, len--) {
+    out[s] = a[0];
+    const int L = len - 1, val = a[L];
+    int hole = 0, child = 0;
+    while (child < (L - 1) / 2) {
+      child = 2 * (child + 1);
+      a[hole] = a[child];
+      hole = child;
+    }
+    if ((L & 1) == 0 && child == (L - 2) / 2) {
+      child = 2 * (child + 1);
+      a[hole] = a[child - 1];
+      hole = child - 1;
+    }
+    if (L) a[hole] = val;
+  }
+}
+
+ORC_API void orc_build_backlinks(uint8_t *level0, uint64_t size_per_elem, uint64_t offset_data, int maxM0, int M,
+                                 int Ks, const float *tables, const uint64_t *sel, const float *dist,
+                                 const int32_t *found, int64_t B, int k, uint32_t first, int queue_order,
+                                 int64_t *counts) {
+  uint32_t *keep = malloc((size_t)maxM0 * sizeof(uint32_t));
+  int *order = malloc((size_t)maxM0 * sizeof(int));
+  for (int64_t i = 0; i < B; i++) {
+    const uint32_t x = first + (uint32_t)i;
+    const float *T = tables + (size_t)i * M * Ks;
+    const int nf = found[i] < k ? found[i] : k;
+    for (int j = 0; j < nf; j++) {
+      const uint32_t r = (uint32_t)sel[(size_t)i * k + j];
+      const float dr = dist[(size_t)i * k + j];
+      uint8_t *rec = level0 + (size_t)r * size_per_elem;
+      uint16_t cnt;
+      memcpy(&cnt, rec, 2);
+      if (cnt < maxM0) {
+        memcpy(rec + 4 + 4 * (size_t)cnt, &x, 4);
+        cnt++;
+        memcpy(rec, &cnt, 2);
+        counts[0]++;
+        continue;
+      }
+      int nk = 0;
+      for (int s = 0; s < cnt; s++) {
+        uint32_t c;
+        memcpy(&c, rec + 4 + 4 * (size_t)s, 4);
+        const uint8_t *code = level0 + (size_t)c * size_per_elem + offset_data;
+        float d = 0.f;
+        for (int m = 0; m < M; m++) d += T[(size_t)m * Ks + code[m]];
+        if (!(d < dr)) {
+          int t = nk++;
+          while (t > 0 && keep[t - 1] < c) { keep[t] = keep[t - 1]; t--; }  /* descending id */
+          keep[t] = c;
+        }
+      }
+      const int total = 1 + nk < maxM0 ? 1 + nk : maxM0;
+      if (queue_order) heap_pop_order(total, order);
+      else for (int s = 0; s < total; s++) order[s] = s;
+      for (int s = 0; s < total; s++) memcpy(rec + 4 + 4 * (size_t)s, order[s] ? &keep[order[s] - 1] : &x, 4);
+      cnt = (uint16_t)total;
+      memcpy(rec, &cnt, 2);
+      counts[1]++;
+      if (1 + nk > maxM0) counts[2]++;
+    }
+  }
+  free(keep);
+  free(order);
 }

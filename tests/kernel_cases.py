@@ -266,18 +266,18 @@ COVERED = set().union(*(c['keys'] for c in CASES))
 
 # ---- kernels of other paths and the tests that run them -------------------------------------------------------------
 ELSEWHERE = {
-    'encode_kernel<u8>': 'tests/test_gpu_parity.py (encode against oracle.encode)',
+    'encode_kernel<u8>': 'tests/test_gpu_parity.py (encode against oracle.encode); tests/test_gpu_build_model.py (built codes)',
     'encode_kernel<u16>': 'tests/test_gpu_wide_codes.py (u16 codes encoded on the device)',
     'l2_normalize_kernel': 'tests/test_gpu_parity.py (cosine queries normalised on the device)',
     'pack_rec0_kernel': 'tests/test_gpu_shapes.py (every search after set_graph / add_items)',
     'scatter_records_kernel': 'tests/test_gpu_build.py (incremental device-graph patches)',
     'mark_labels_kernel': 'tests/test_gpu_walk4f.py (filter_labels -> bitmap)',
     'gather_filter_kernel': 'tests/test_gpu_walk4f.py (filter_labels -> bitmap)',
-    'export_links_kernel': 'tests/test_gpu_build.py (GPU builder)',
-    'link_new_nodes_kernel': 'tests/test_gpu_build.py (GPU builder)',
-    'reverse_link_kernel': 'tests/test_gpu_build.py (GPU builder)',
-    'link_new_nodes_cells_kernel': 'tests/test_gpu_cells_build.py (one-pass cell-set build)',
-    'reverse_link_cells_kernel': 'tests/test_gpu_cells_build.py (one-pass cell-set build)',
+    'export_links_kernel': 'tests/test_gpu_build_model.py (GPU builder byte for byte against the build model)',
+    'link_new_nodes_kernel': 'tests/test_gpu_build_model.py (GPU builder byte for byte against the build model)',
+    'reverse_link_kernel': 'tests/test_gpu_build_model.py (GPU builder byte for byte against the build model)',
+    'link_new_nodes_cells_kernel': 'tests/test_gpu_build_model.py (one-pass cell-set build against the build model)',
+    'reverse_link_cells_kernel': 'tests/test_gpu_build_model.py (one-pass cell-set build against the build model)',
     'filter_eval_kernel<0>': 'tests/test_gpu_attr_filter.py (attribute filters)',
     'filter_eval_kernel<1>': 'tests/test_gpu_attr_filter.py (attribute filters)',
     'rows_copy_kernel': 'tests/test_gpu_attr_filter.py (attribute columns)',
