@@ -136,7 +136,9 @@ def check(rc):
         return
     msg = load().annb_last_error().decode('utf-8', 'replace')
     if rc == EINVAL:
-        raise ValueError(msg) if 'Initialization Error' in msg else AnnbError(rc, msg)
+        # a bad codec geometry, and a batch with a NaN or an infinity (scipy.cluster.vq's ValueError in the reference)
+        refused = 'Initialization Error' in msg or 'must not contain infs or NaNs' in msg
+        raise ValueError(msg) if refused else AnnbError(rc, msg)
     if rc == ENOMEM:
         raise MemoryError(msg)
     if rc == ELIMIT and 'PQ clustering exceed' in msg:

@@ -97,7 +97,8 @@ class PQCodec:
 
     # ---- encode / decode ------------------------------------------------------------------------
     def encode(self, x: 'np.ndarray'):
-        """pq.py:158-177 on the device (nearest codeword per subspace, first minimum)."""
+        """pq.py:158-177 on the device (nearest codeword per subspace, first minimum).  Rows with a NaN or an
+        infinity raise ValueError, as scipy.cluster.vq does in the reference."""
         assert x.dtype == np.float32 and x.ndim == 2
         assert x.shape[1] == self.d_subvector * self.n_subvectors, 'input dimension must be Ds * M'
         return self.engine.encode(x).astype(self.code_dtype, copy=False)

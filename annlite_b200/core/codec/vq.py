@@ -71,7 +71,8 @@ class VQCodec:
     # ---- encode (vq.py:75-82: scipy.cluster.vq.vq on the raw vectors, Euclidean whatever the metric) -------------
     def encode(self, x: 'np.ndarray'):
         """Each row's nearest centroid (first minimum), int32.  scipy's rounding is not reproduced bit for bit: rows
-        whose two nearest centroids are within rounding of each other may be routed to the other one."""
+        whose two nearest centroids are within rounding of each other may be routed to the other one.  Rows with a NaN
+        or an infinity raise ValueError, as scipy.cluster.vq does."""
         self._check_trained()
         assert x.dtype == np.float32 and x.ndim == 2
         if self._engine is None:

@@ -20,10 +20,13 @@ namespace {
 constexpr int K1_THREADS = 256;
 constexpr int K1_QT = 32;  // queries per CTA
 
-template <int DS>  // DS > 0: compile-time subvector length, codeword in registers; DS == 0: runtime ds
+// DS > 0: compile-time subvector length, codeword in registers.  DS == 0: runtime ds; with `staged` the query tile and
+// the CTA's codewords are copied to shared memory first, without it (ds too large for them to fit) both are read from
+// global memory, where the codebook is L2 resident.  The arithmetic is the same either way.
+template <int DS>
 __global__ void __launch_bounds__(K1_THREADS)
 adc_table_kernel(const float *__restrict__ q, const float *__restrict__ cb, float *__restrict__ out,
-                 int64_t B, int M, int Ks, int ds_rt, int is_ip, float bias) {
+                 int64_t B, int M, int Ks, int ds_rt, int is_ip, float bias, int staged) {
   extern __shared__ float sm[];  // [K1_QT][ds] query sub-vectors, then (DS==0) [K1_THREADS][ds+1] codewords
   const int ds = DS > 0 ? DS : ds_rt;
   const int D = M * ds;
@@ -33,26 +36,31 @@ adc_table_kernel(const float *__restrict__ q, const float *__restrict__ cb, floa
   const int64_t b0 = (int64_t)blockIdx.y * K1_QT;
   const int nq = (int)min((int64_t)K1_QT, B - b0);
 
-  float *qs = sm;
-  for (int i = threadIdx.x; i < nq * ds; i += K1_THREADS) {
-    int qi = i / ds, j = i - qi * ds;
-    qs[i] = q[(b0 + qi) * D + (int64_t)m * ds + j];
-  }
+  const bool smem = DS > 0 || staged;
+  const float *qs = smem ? sm : q + b0 * D + (int64_t)m * ds;
+  const int qstride = smem ? ds : D;
+  if (smem)
+    for (int i = threadIdx.x; i < nq * ds; i += K1_THREADS) {
+      int qi = i / ds, j = i - qi * ds;
+      sm[i] = q[(b0 + qi) * D + (int64_t)m * ds + j];
+    }
   float cw[DS > 0 ? DS : 1];
-  float *cws = sm + K1_QT * ds + threadIdx.x * (ds + 1);
+  const float *cws = sm + K1_QT * ds + threadIdx.x * (ds + 1);
   if (c < Ks) {
     const float *w = cb + ((size_t)m * Ks + c) * ds;
     if (DS > 0) {
 #pragma unroll
       for (int j = 0; j < DS; j++) cw[j] = w[j];
+    } else if (staged) {
+      for (int j = 0; j < ds; j++) sm[K1_QT * ds + threadIdx.x * (ds + 1) + j] = w[j];
     } else {
-      for (int j = 0; j < ds; j++) cws[j] = w[j];
+      cws = w;
     }
   }
-  __syncthreads();
+  if (smem) __syncthreads();
   if (c >= Ks) return;
   for (int qi = 0; qi < nq; qi++) {
-    const float *x = qs + qi * ds;
+    const float *x = qs + qi * qstride;
     float acc = 0.f;
     if (DS > 0) {
 #pragma unroll
@@ -96,19 +104,31 @@ __global__ void l2_normalize_kernel(float *__restrict__ x, int64_t B, int D) {
   for (int j = lane; j < D; j += 32) r[j] = __fdiv_rn(r[j], nrm);
 }
 
-// PQCodec.encode (annlite/core/codec/pq.py:158-177): nearest codeword per subspace, first
-// minimum.  One warp per (row, subspace); lanes stride over codewords, fp32 squared distance
-// with sequential j (the reference delegates to scipy.cluster.vq.vq whose rounding is BLAS
-// dependent, so parity here is a mismatch *rate* on near-ties; SURVEY.md section 8f rank 1).
+// PQCodec.encode (annlite/core/codec/pq.py:158-177): nearest codeword per subspace, first minimum.  One warp per
+// (row, subspace); lanes stride over codewords, fp32 squared distance with sequential j.  The reference delegates to
+// scipy.cluster.vq.vq, whose rounding is BLAS dependent, so the chosen codeword is checked against a float64 argmin
+// with a rounding bound (tests/numeric_bounds.py), not bit for bit.
+// One order, `precedes`, serves the lane loop and the shuffle reduction: NaN counts as +inf and equal values go to
+// the lower index.  A lane starts neutral (+inf, no index) and takes its first codeword whatever its distance, so
+// the code is always < Ks and a row whose every distance overflows to +inf encodes to 0.  scipy refuses non-finite
+// rows; a row with a NaN or +-inf coordinate lowers *bad_row to its index (when bad_row is given), so the caller can
+// refuse the batch before it uses the codes.
+__device__ __forceinline__ bool precedes(float a, int ia, float b, int ib) { return a < b || (a == b && ia < ib); }
+
 template <typename code_t>
-__global__ void encode_kernel(const float *__restrict__ x, const float *__restrict__ cb,
-                              code_t *__restrict__ codes, int64_t N, int M, int Ks, int ds) {
+__global__ void encode_kernel(const float *__restrict__ x, const float *__restrict__ cb, code_t *__restrict__ codes,
+                              int64_t N, int M, int Ks, int ds, unsigned long long *__restrict__ bad_row) {
   const int64_t wid = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (wid >= N * M) return;
   const int64_t n = wid / M;
   const int m = (int)(wid - n * M);
   const float *v = x + n * (int64_t)M * ds + (int64_t)m * ds;
+  if (bad_row) {
+    bool bad = false;
+    for (int j = lane; j < ds; j += 32) bad |= !isfinite(v[j]);
+    if (__any_sync(0xffffffffu, bad) && lane == 0) atomicMin(bad_row, (unsigned long long)n);
+  }
   float best = CUDART_INF_F;
   int arg = 0x7fffffff;
   for (int c = lane; c < Ks; c += 32) {
@@ -118,7 +138,8 @@ __global__ void encode_kernel(const float *__restrict__ x, const float *__restri
       float t = __fsub_rn(v[j], w[j]);
       acc = __fadd_rn(acc, __fmul_rn(t, t));
     }
-    if (acc < best) {
+    if (isnan(acc)) acc = CUDART_INF_F;
+    if (precedes(acc, c, best, arg)) {
       best = acc;
       arg = c;
     }
@@ -127,7 +148,7 @@ __global__ void encode_kernel(const float *__restrict__ x, const float *__restri
   for (int o = 16; o > 0; o >>= 1) {
     float ob = __shfl_xor_sync(0xffffffffu, best, o);
     int oa = __shfl_xor_sync(0xffffffffu, arg, o);
-    if (ob < best || (ob == best && oa < arg)) {
+    if (precedes(ob, oa, best, arg)) {
       best = ob;
       arg = oa;
     }
@@ -162,7 +183,7 @@ int launch_adc_table(annb_index *h, const float *d_queries, int64_t B, float *d_
 #define K1_CASE(DSV)                                                                                   \
   case DSV:                                                                                            \
     adc_table_kernel<DSV><<<grid, K1_THREADS, sm_q, h->stream>>>(q, h->d_codebook, o, nb, h->M, h->Ks, \
-                                                                  h->ds, is_ip, bias);                 \
+                                                                  h->ds, is_ip, bias, 1);              \
     break;
     switch (h->ds) {
       K1_CASE(2)
@@ -174,11 +195,16 @@ int launch_adc_table(annb_index *h, const float *d_queries, int64_t B, float *d_
       K1_CASE(24)
       K1_CASE(32)
       default: {
+        // the query tile and the codewords in shared memory while they fit (ds <= 200 on H100), else neither
         size_t smb = sm_q + (size_t)K1_THREADS * (h->ds + 1) * sizeof(float);
+        int optin = 0;
+        ANNB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+        const int staged = smb <= (size_t)optin;
+        if (!staged) smb = 0;
         if (smb > 48 * 1024)
           ANNB_CUDA(cudaFuncSetAttribute(adc_table_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smb));
         adc_table_kernel<0><<<grid, K1_THREADS, smb, h->stream>>>(q, h->d_codebook, o, nb, h->M, h->Ks, h->ds,
-                                                                 is_ip, bias);
+                                                                 is_ip, bias, staged);
       }
     }
 #undef K1_CASE
@@ -189,15 +215,18 @@ int launch_adc_table(annb_index *h, const float *d_queries, int64_t B, float *d_
   return ANNB_OK;
 }
 
-int launch_encode(annb_index *h, const float *d_x, int64_t n, void *d_codes) {
+int launch_encode(annb_index *h, const float *d_x, int64_t n, void *d_codes, unsigned long long *d_bad_row) {
   if (n == 0) return ANNB_OK;
   const int warps = 8;
   int64_t total = n * h->M;
   unsigned grid = (unsigned)((total + warps - 1) / warps);
+  if (d_bad_row) ANNB_CUDA(cudaMemsetAsync(d_bad_row, 0xff, sizeof(unsigned long long), h->stream));
   if (h->code_bytes == 1)
-    encode_kernel<uint8_t><<<grid, warps * 32, 0, h->stream>>>(d_x, h->d_codebook, (uint8_t *)d_codes, n, h->M, h->Ks, h->ds);
+    encode_kernel<uint8_t><<<grid, warps * 32, 0, h->stream>>>(d_x, h->d_codebook, (uint8_t *)d_codes, n, h->M, h->Ks, h->ds,
+                                                                d_bad_row);
   else
-    encode_kernel<uint16_t><<<grid, warps * 32, 0, h->stream>>>(d_x, h->d_codebook, (uint16_t *)d_codes, n, h->M, h->Ks, h->ds);
+    encode_kernel<uint16_t><<<grid, warps * 32, 0, h->stream>>>(d_x, h->d_codebook, (uint16_t *)d_codes, n, h->M, h->Ks,
+                                                                 h->ds, d_bad_row);
   h->launches++;
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;

@@ -367,7 +367,11 @@ int launch_l2_normalize(annb_index *h, float *x, int64_t B, int D);
 int launch_adc_table(annb_index *h, const float *d_queries, int64_t B, float *d_out);
 int launch_scan(annb_index *h, const float *d_table, float *d_out);
 int launch_scan_topk(annb_index *h, const float *d_tables, int64_t B, int k, int64_t *d_ids, float *d_dists);
-int launch_encode(annb_index *h, const float *d_x, int64_t n, void *d_codes);
+// d_bad_row (or nullptr): set to the first row holding a NaN or an infinity, ~0 if none (reset on h->stream first)
+int launch_encode(annb_index *h, const float *d_x, int64_t n, void *d_codes, unsigned long long *d_bad_row);
+// ANNB_EINVAL naming the first row of host rows (n, dim) that holds a NaN or an infinity
+int check_finite_rows(const float *v, int64_t n, int dim);
+#define ANNB_NONFINITE_MSG "array must not contain infs or NaNs"
 int launch_pack_rec0(annb_index *h, const uint8_t *d_level0_raw, int64_t n);
 int launch_scatter_records(annb_index *h, const uint8_t *d_staged, const uint32_t *d_ids, int64_t cnt, int rec_bytes, uint8_t *d_dst);
 // mode: 0 = fast walk (no filter, no deletions), 1 = filtered/deleted walk, kernel chosen automatically

@@ -596,14 +596,18 @@ int annb_encode(annb_index_t *h, const float *vectors, int v_space, int64_t n, v
   if (n == 0) return ANNB_OK;
   const float *dx;
   ANNB_TRY(stage_in(h, vectors, v_space, (size_t)n * h->dim * sizeof(float), S_QUERIES, (const void **)&dx));
-  void *dc = codes;
-  const size_t cbytes = (size_t)n * h->M * h->code_bytes;
-  if (c_space != ANNB_DEVICE) ANNB_TRY(annb_scratch(h, S_CODES, cbytes, &dc));
-  ANNB_TRY(launch_encode(h, dx, n, dc));
-  if (c_space != ANNB_DEVICE) {
-    ANNB_CUDA(cudaMemcpyAsync(codes, dc, cbytes, cudaMemcpyDeviceToHost, h->stream));
-    ANNB_CUDA(cudaStreamSynchronize(h->stream));
-  }
+  // codes into scratch, the first non-finite row behind them: the caller's codes are written only for a finite batch
+  const size_t cbytes = (size_t)n * h->M * h->code_bytes, flag_at = (cbytes + 7) / 8 * 8;
+  uint8_t *dc;
+  ANNB_TRY(annb_scratch(h, S_CODES, flag_at + sizeof(unsigned long long), (void **)&dc));
+  unsigned long long *d_bad = reinterpret_cast<unsigned long long *>(dc + flag_at), bad = 0;
+  ANNB_TRY(launch_encode(h, dx, n, dc, d_bad));
+  ANNB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(bad), cudaMemcpyDeviceToHost, h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  if (bad != ~0ull) ANNB_FAIL(ANNB_EINVAL, "row %llu holds a NaN or an infinity: %s", bad, ANNB_NONFINITE_MSG);
+  ANNB_CUDA(cudaMemcpyAsync(codes, dc, cbytes, c_space == ANNB_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                            h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
   return ANNB_OK;
 }
 
@@ -657,6 +661,7 @@ int annb_add_items(annb_index_t *h, const float *vectors, const void *codes, con
   if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
   if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised: call annb_init_graph first");
   if (n == 0) return ANNB_OK;
+  ANNB_TRY(check_finite_rows(vectors, n, h->dim));
   h->state_gen++;
   ANNB_CUDA(cudaStreamSynchronize(h->stream));   // insertion reuses search scratch: let streamed searches finish
   ANNB_CUDA(cudaStreamSynchronize(h->stream2));
@@ -670,6 +675,19 @@ int annb_add_items(annb_index_t *h, const float *vectors, const void *codes, con
 }
 
 }  // extern "C"
+
+// The first row of a host batch (n, dim) holding a NaN or an infinity refuses the batch: a PQ code or a cell cannot be
+// chosen for it (scipy.cluster.vq refuses it too).  Insertions check their rows here, before anything is written: the
+// GPU builder inserts its first rows on the host before it encodes the rest.
+int check_finite_rows(const float *v, int64_t n, int dim) {
+  for (int64_t i = 0; i < n; i++) {
+    const uint32_t *r = reinterpret_cast<const uint32_t *>(v + (size_t)i * dim);
+    uint32_t bad = 0;
+    for (int j = 0; j < dim; j++) bad |= (r[j] & 0x7f800000u) == 0x7f800000u;
+    if (bad) ANNB_FAIL(ANNB_EINVAL, "row %lld holds a NaN or an infinity: %s", (long long)i, ANNB_NONFINITE_MSG);
+  }
+  return ANNB_OK;
+}
 
 int hnsw_host_add(annb_index *h, const float *vectors, const void *codes, const uint64_t *labels, int64_t n, int num_threads,
                   const int32_t *forced_levels) {
@@ -688,7 +706,7 @@ int hnsw_host_add(annb_index *h, const float *vectors, const void *codes, const 
       ANNB_TRY(annb_scratch(h, S_QUERIES, (size_t)c * h->dim * sizeof(float), (void **)&dx));
       ANNB_TRY(annb_scratch(h, S_CODES, (size_t)c * crow, &dc));
       ANNB_CUDA(cudaMemcpyAsync(dx, vectors + (size_t)s * h->dim, (size_t)c * h->dim * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-      ANNB_TRY(launch_encode(h, dx, c, dc));
+      ANNB_TRY(launch_encode(h, dx, c, dc, nullptr));  // annb_add_items checked the rows
       ANNB_CUDA(cudaMemcpyAsync(own_codes.data() + (size_t)s * crow, dc, (size_t)c * crow, cudaMemcpyDeviceToHost, h->stream));
       ANNB_CUDA(cudaStreamSynchronize(h->stream));
     }

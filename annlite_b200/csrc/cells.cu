@@ -1282,6 +1282,7 @@ int annb_cellset_add_items(annb_cellset_t *cs, const float *vectors, const uint6
   if (!cs) ANNB_FAIL(ANNB_EINVAL, "null cell set");
   if (n < 0 || (n > 0 && (!vectors || !labels || !cells))) ANNB_FAIL(ANNB_EINVAL, "null vectors/labels/cells");
   const int C = cs->n_cells;
+  if (n > 0) ANNB_TRY_RC(check_finite_rows(vectors, n, cs->dim));
   std::vector<std::vector<int64_t>> rows((size_t)C);
   for (int64_t i = 0; i < n; i++) {
     const int32_t c = cells[i];

@@ -447,7 +447,7 @@ int gpu_build_run(annb_index *h, const float *vectors, const uint64_t *labels, i
     ANNB_CUDA(cudaMemcpyAsync(dq, hq, (size_t)B * dim * 4, cudaMemcpyHostToDevice, h->stream));
     ANNB_CUDA(cudaMemcpyAsync(dlab, hlab, (size_t)B * 8, cudaMemcpyHostToDevice, h->stream));
     // the reference encodes the row as handed in and builds its table from the re-normalised row (pq.py:309-310)
-    ANNB_TRY_RC(launch_encode(h, dq, B, b.node_codes + (size_t)n_cur * M));
+    ANNB_TRY_RC(launch_encode(h, dq, B, b.node_codes + (size_t)n_cur * M, nullptr));
     if (h->metric == ANNB_METRIC_COSINE) ANNB_TRY_RC(launch_l2_normalize(h, dq, B, dim));
     SearchParams sp;
     memset(&sp, 0, sizeof(sp));
@@ -706,7 +706,8 @@ int gpu_build_cells(annb_index *drv, std::vector<CellBuildJob> &jobs, int num_th
     // encode each cell's segment into its node codes (the cells share the codebook), then normalise once for cosine:
     // the reference encodes the row as handed in and builds its table from the re-normalised row (pq.py:309-310)
     for (int e = 0; e < E; e++)
-      if (Bc[e]) ANNB_TRY_RC(launch_encode(drv, dq + (size_t)off[e] * dim, Bc[e], cs[e].b.node_codes + (size_t)cs[e].n_cur * M));
+      if (Bc[e]) ANNB_TRY_RC(launch_encode(drv, dq + (size_t)off[e] * dim, Bc[e], cs[e].b.node_codes + (size_t)cs[e].n_cur * M,
+                                                   nullptr));
     if (drv->metric == ANNB_METRIC_COSINE) ANNB_TRY_RC(launch_l2_normalize(drv, dq, R, dim));
     for (int e = 0; e < E; e++) {
       gdh[e] = jobs[e].h->gd;

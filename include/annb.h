@@ -163,7 +163,9 @@ ANNB_API int annb_get_graph(annb_index_t *h, uint8_t *data_level0, uint8_t *link
  * each row's ADC table on the fly (the reference materialises (n,M,Ks) tables; this does not)
  * and inserts with the reference's algorithm, including its PQ-mode neighbour heuristic
  * (SURVEY.md section 0.2).  num_threads == 1 reproduces the reference's single-threaded graph
- * bit for bit; > 1 inserts concurrently like ParallelFor (hnsw_bindings.cpp:24-77). */
+ * bit for bit; > 1 inserts concurrently like ParallelFor (hnsw_bindings.cpp:24-77).  A batch with a
+ * NaN or an infinity in any row is refused (ANNB_EINVAL naming the first such row) before anything
+ * is inserted. */
 ANNB_API int annb_add_items(annb_index_t *h, const float *vectors, const void *codes, const uint64_t *labels,
                    int64_t n, int num_threads);
 
@@ -174,7 +176,11 @@ ANNB_API int annb_add_items(annb_index_t *h, const float *vectors, const void *c
 ANNB_API int annb_add_items_with_tables(annb_index_t *h, const void *codes, const float *tables,
                                const uint64_t *labels, int64_t n, int num_threads);
 
-/* PQCodec.encode (pq.py:158-177): nearest codeword per subspace, first minimum. (n,dim)->(n,M). */
+/* PQCodec.encode (pq.py:158-177): nearest codeword per subspace, first minimum. (n,dim)->(n,M).
+ * A NaN distance counts as +inf and equal distances go to the lower index, so every code is below
+ * n_clusters (a subspace whose every distance overflows takes codeword 0).  A batch with a NaN or
+ * an infinity in any row is refused (ANNB_EINVAL naming the first such row); `codes` is then not
+ * written. */
 ANNB_API int annb_encode(annb_index_t *h, const float *vectors, int v_space, int64_t n, void *codes, int c_space);
 
 ANNB_API int annb_resize_index(annb_index_t *h, int64_t new_max_elements); /* hnswalg.h:680-706           */
@@ -475,7 +481,8 @@ ANNB_API int annb_cellset_last_ms(annb_cellset_t *cs, float *probe_ms, float *wa
  * would pick), with one multi-cell walk launch per round (more when a round's by-cell scratch would pass 256 MB or the
  * cells' ef_construction differ), one encode launch per cell, and two link launches.  Every other share is
  * annb_add_items on its own handle.  Every share is checked first: an error names the cell, and a share that would
- * overrun its cell's capacity gives ANNB_ECAPACITY before anything is inserted. */
+ * overrun its cell's capacity gives ANNB_ECAPACITY before anything is inserted, a row with a NaN or an infinity
+ * ANNB_EINVAL naming it. */
 ANNB_API int annb_cellset_add_items(annb_cellset_t *cs, const float *vectors, const uint64_t *labels, const int32_t *cells,
                            int64_t n, int num_threads);
 /* The last annb_cellset_add_items' one-pass build: host time of phase 1 and of phase 2 with the host graphs'

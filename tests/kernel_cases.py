@@ -266,9 +266,9 @@ COVERED = set().union(*(c['keys'] for c in CASES))
 
 # ---- kernels of other paths and the tests that run them -------------------------------------------------------------
 ELSEWHERE = {
-    'encode_kernel<u8>': 'tests/test_gpu_parity.py (encode against oracle.encode); tests/test_gpu_build_model.py (built codes)',
-    'encode_kernel<u16>': 'tests/test_gpu_wide_codes.py (u16 codes encoded on the device)',
-    'l2_normalize_kernel': 'tests/test_gpu_parity.py (cosine queries normalised on the device)',
+    'encode_kernel<u8>': 'tests/test_gpu_numeric_edges.py (codes against the float64 argmin rule, ties, overflow, refusals)',
+    'encode_kernel<u16>': 'tests/test_gpu_numeric_edges.py (u16 codes against the float64 argmin rule, ties, overflow)',
+    'l2_normalize_kernel': 'tests/test_gpu_numeric_edges.py (normalised rows against the float64 rule and its switch)',
     'pack_rec0_kernel': 'tests/test_gpu_shapes.py (every search after set_graph / add_items)',
     'scatter_records_kernel': 'tests/test_gpu_build.py (incremental device-graph patches)',
     'mark_labels_kernel': 'tests/test_gpu_walk4f.py (filter_labels -> bitmap)',
@@ -286,7 +286,7 @@ ELSEWHERE = {
     'filter_count_kernel': 'tests/test_gpu_attr_filter.py (filter_labels of a prepared filter)',
     'cell_scatter_kernel': 'tests/test_gpu_cells.py (per-cell parts of the fused cell-set walk)',
     'ivf_merge_kernel': 'tests/test_gpu_cells.py (merged cell-set rows against oracle/ivf.py)',
-    'cell_probe_kernel': 'tests/test_gpu_cells.py (GPU probe order against cdist)',
+    'cell_probe_kernel': 'tests/test_gpu_numeric_edges.py (every adjacent pair of the probe order, float64 rule)',
     'subset_count_kernel': 'tests/test_gpu_cells_bruteforce.py (attribute-filter bitmaps scanned exactly)',
     'subset_offsets_kernel': 'tests/test_gpu_cells_bruteforce.py (attribute-filter bitmaps scanned exactly)',
 }
