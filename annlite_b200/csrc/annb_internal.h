@@ -430,13 +430,17 @@ int launch_merge_topk(annb_index *h, const uint64_t *labels, const float *dists,
 int launch_filter_bitmap(annb_index *h, const uint64_t *d_filter_labels, int64_t n_filter, uint32_t *d_by_label,
                          uint32_t *d_by_id);
 // attr_filter.cu: evaluate a validated program over rows [0, n) into a by-id bitmap ((n+31)/32 + 1 words) and its
-// admitted count (device u64, accumulated: the caller zeroes it); compact a bitmap into the labels of its rows
+// admitted count (device u64, accumulated: the caller zeroes it); compact a bitmap, less the rows set in d_drop
+// (nullable), into the labels of its rows
 int launch_filter_eval(annb_index *h, const annb_filter_op_t *d_prog, int n_ops, const void *d_consts, int n_const_bytes,
                        const AttrColDev *cols, int n_cols, int64_t n, const uint32_t *d_deleted, uint32_t *d_bits,
                        unsigned long long *d_count);
-int launch_filter_compact(annb_index *h, const uint32_t *d_bits, int64_t n, const uint64_t *d_labels, uint64_t *d_out,
-                          unsigned int *d_block_scratch);
-// blocks launch_filter_compact uses for n rows (its scratch holds one u32 per block)
+// in two steps: launch_filter_count leaves each block's offset in d_block_scratch and the total after them;
+// launch_filter_compact then writes that many labels to d_out
+int launch_filter_count(annb_index *h, const uint32_t *d_bits, const uint32_t *d_drop, int64_t n, unsigned int *d_block_scratch);
+int launch_filter_compact(annb_index *h, const uint32_t *d_bits, const uint32_t *d_drop, int64_t n, const uint64_t *d_labels,
+                          uint64_t *d_out, const unsigned int *d_block_scratch);
+// blocks the compaction uses for n rows (its scratch holds one u32 per block, plus the total)
 int64_t filter_compact_blocks(int64_t n);
 // F validated programs in one pass (filter_eval_kernel<true>): program f = ops [d_offs[f], d_offs[f + 1]) of d_prog,
 // constant offsets rebased into the one pool; bitmap f at d_bits + f * stride_words, its count added to d_counts[f]

@@ -11,7 +11,8 @@
 // the other over its 32 rows, so HBM sees about one pass over the referenced columns plus F * n / 8 bytes of bitmaps.
 //
 // filter_compact_kernel turns a bitmap into the labels of its rows in internal-id order: per-block counts, one scan
-// of the block counts, then each block writes its rows at its offset.
+// of the block counts (which also leaves the total behind them), then each block writes its rows at its offset.  An
+// optional `drop` bitmap (the deletions) is masked out of every word on the way.
 #include <algorithm>
 #include <cstring>
 
@@ -197,18 +198,23 @@ __device__ __forceinline__ unsigned int block_exclusive_scan(unsigned int v, uns
   return before + x - v;
 }
 
+__device__ __forceinline__ uint32_t listed_word(const uint32_t *bits, const uint32_t *drop, int64_t w, int64_t nwords) {
+  return w < nwords ? bits[w] & ~(drop ? drop[w] : 0u) : 0u;
+}
+
 // pass 1: admitted rows per block
-__global__ void __launch_bounds__(kCompactThreads) filter_count_kernel(const uint32_t *__restrict__ bits, int64_t nwords,
+__global__ void __launch_bounds__(kCompactThreads) filter_count_kernel(const uint32_t *__restrict__ bits,
+                                                                       const uint32_t *__restrict__ drop, int64_t nwords,
                                                                        unsigned int *__restrict__ block_counts) {
   __shared__ unsigned int warp_sums[kCompactThreads / 32];
   const int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned int c = w < nwords ? __popc(bits[w]) : 0u;
+  const unsigned int c = __popc(listed_word(bits, drop, w, nwords));
   unsigned int total;
   block_exclusive_scan(c, warp_sums, &total);
   if (threadIdx.x == 0) block_counts[blockIdx.x] = total;
 }
 
-// pass 2: exclusive scan of the block counts, in place (one block)
+// pass 2: exclusive scan of the block counts, in place (one block); the total goes to block_counts[nblocks]
 __global__ void __launch_bounds__(1024) filter_scan_kernel(unsigned int *__restrict__ block_counts, int64_t nblocks) {
   __shared__ unsigned int warp_sums[32];
   __shared__ unsigned int carry;
@@ -224,16 +230,18 @@ __global__ void __launch_bounds__(1024) filter_scan_kernel(unsigned int *__restr
     if (threadIdx.x == 0) carry += total;
     __syncthreads();
   }
+  if (threadIdx.x == 0) block_counts[nblocks] = carry;
 }
 
 // pass 3: each block writes the labels of its admitted rows at its offset, in internal-id order
-__global__ void __launch_bounds__(kCompactThreads) filter_compact_kernel(const uint32_t *__restrict__ bits, int64_t nwords,
+__global__ void __launch_bounds__(kCompactThreads) filter_compact_kernel(const uint32_t *__restrict__ bits,
+                                                                         const uint32_t *__restrict__ drop, int64_t nwords,
                                                                          const unsigned int *__restrict__ block_offsets,
                                                                          const uint64_t *__restrict__ labels,
                                                                          uint64_t *__restrict__ out) {
   __shared__ unsigned int warp_sums[kCompactThreads / 32];
   const int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t word = w < nwords ? bits[w] : 0u;
+  uint32_t word = listed_word(bits, drop, w, nwords);
   unsigned int pos = block_offsets[blockIdx.x] + block_exclusive_scan(__popc(word), warp_sums, nullptr);
   while (word) {
     const int b = __ffs(word) - 1;
@@ -307,14 +315,20 @@ int64_t filter_compact_blocks(int64_t n) {
   return std::max<int64_t>(1, (nwords + kCompactThreads - 1) / kCompactThreads);
 }
 
-int launch_filter_compact(annb_index *h, const uint32_t *d_bits, int64_t n, const uint64_t *d_labels, uint64_t *d_out,
-                          unsigned int *d_block_scratch) {
-  const int64_t nwords = (n + 31) / 32;
+int launch_filter_count(annb_index *h, const uint32_t *d_bits, const uint32_t *d_drop, int64_t n, unsigned int *d_block_scratch) {
   const int64_t nb = filter_compact_blocks(n);
-  filter_count_kernel<<<(unsigned)nb, kCompactThreads, 0, h->stream>>>(d_bits, nwords, d_block_scratch);
+  filter_count_kernel<<<(unsigned)nb, kCompactThreads, 0, h->stream>>>(d_bits, d_drop, (n + 31) / 32, d_block_scratch);
   filter_scan_kernel<<<1, 1024, 0, h->stream>>>(d_block_scratch, nb);
-  filter_compact_kernel<<<(unsigned)nb, kCompactThreads, 0, h->stream>>>(d_bits, nwords, d_block_scratch, d_labels, d_out);
-  h->launches += 3;
+  h->launches += 2;
+  ANNB_CUDA(cudaGetLastError());
+  return ANNB_OK;
+}
+
+int launch_filter_compact(annb_index *h, const uint32_t *d_bits, const uint32_t *d_drop, int64_t n, const uint64_t *d_labels,
+                          uint64_t *d_out, const unsigned int *d_block_scratch) {
+  filter_compact_kernel<<<(unsigned)filter_compact_blocks(n), kCompactThreads, 0, h->stream>>>(d_bits, d_drop, (n + 31) / 32,
+                                                                                              d_block_scratch, d_labels, d_out);
+  h->launches++;
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;
 }

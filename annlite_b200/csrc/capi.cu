@@ -1796,6 +1796,24 @@ static int validate_program(const annb_index *h, const annb_filter_op_t *prog, i
     if (o.op != ANNB_FOP_NOTNULL && (o.a < 0 || o.a % align || (int64_t)o.a + need > n_const_bytes))
       ANNB_FAIL(ANNB_EINVAL, "filter op %d: constants [%d, %lld) outside the pool of %lld bytes or misaligned", i, o.a,
                 (long long)o.a + need, (long long)n_const_bytes);
+    // the evaluator's membership test is a binary search: a list must be non-decreasing, and a FLOAT one free of NaN
+    const bool int_list = o.op == ANNB_FOP_INT_IN || o.op == ANNB_FOP_INT_NIN;
+    if (int_list || o.op == ANNB_FOP_FLT_IN || o.op == ANNB_FOP_FLT_NIN) {
+      const uint8_t *k = (const uint8_t *)consts + o.a;
+      for (int j = 0; j < o.b; j++) {
+        int64_t iv, ip = 0;
+        double dv, dp = 0.0;
+        memcpy(&iv, k + 8 * j, 8);
+        memcpy(&dv, k + 8 * j, 8);
+        if (j) {
+          memcpy(&ip, k + 8 * (j - 1), 8);
+          memcpy(&dp, k + 8 * (j - 1), 8);
+        }
+        if (!int_list && std::isnan(dv)) ANNB_FAIL(ANNB_EINVAL, "filter op %d (op code %d): list entry %d is NaN", i, o.op, j);
+        if (j && (int_list ? iv < ip : dv < dp))
+          ANNB_FAIL(ANNB_EINVAL, "filter op %d (op code %d): list is not sorted ascending at entry %d", i, o.op, j);
+      }
+    }
   }
   if (depth != 1) ANNB_FAIL(ANNB_EINVAL, "filter program leaves %d values on the stack (must be 1)", depth);
   return ANNB_OK;
@@ -2170,20 +2188,32 @@ int annb_filter_prepare_labels(annb_index_t *h, const uint64_t *labels, int64_t 
   return ANNB_OK;
 }
 
+// The rows listed are the bitmap's.  A program's bitmap already excludes deleted rows; a label list's bitmap holds
+// every row the list names (the walks test deletions separately), so its deleted rows are masked out here.  Only
+// the entries the compaction wrote are copied: their number comes back from the device before anything is copied.
 int annb_filter_labels(annb_index_t *h, int filter_id, uint64_t *labels_out, int64_t cap, int64_t *n_out) {
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
   if (cap < 0 || (cap > 0 && !labels_out)) ANNB_FAIL(ANNB_EINVAL, "bad output buffer");
   PreparedFilter *f;
   ANNB_TRY(find_filter(h, filter_id, &f));
-  if (n_out) *n_out = f->count;
-  const int64_t m = std::min(cap, f->count);
-  if (m == 0) return ANNB_OK;
-  unsigned int *dscan;
+  if (n_out) *n_out = 0;
+  // at most this many rows are listed: a program's count, or a label list's entries that name live rows
+  const int64_t bound = std::min(f->n, f->ids ? f->n_ids : f->count);
+  if (bound == 0) return ANNB_OK;
+  const uint32_t *drop = f->ids ? h->gd.deleted : nullptr;
+  const int64_t nb = filter_compact_blocks(f->n);
+  unsigned int *dscan, total = 0;
   uint64_t *dout;
-  ANNB_TRY(annb_scratch(h, S_FILTER_SCAN, (size_t)filter_compact_blocks(f->n) * 4, (void **)&dscan));
-  ANNB_TRY(annb_scratch(h, S_FILTER_OUT, (size_t)f->count * 8, (void **)&dout));
-  ANNB_TRY(launch_filter_compact(h, f->bits, f->n, h->d_labels, dout, dscan));
+  ANNB_TRY(annb_scratch(h, S_FILTER_SCAN, (size_t)(nb + 1) * 4, (void **)&dscan));
+  ANNB_TRY(launch_filter_count(h, f->bits, drop, f->n, dscan));
+  ANNB_CUDA(cudaMemcpyAsync(&total, dscan + nb, 4, cudaMemcpyDeviceToHost, h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  if (n_out) *n_out = total;
+  const int64_t m = std::min<int64_t>(cap, total);
+  if (m == 0) return ANNB_OK;
+  ANNB_TRY(annb_scratch(h, S_FILTER_OUT, (size_t)total * 8, (void **)&dout));
+  ANNB_TRY(launch_filter_compact(h, f->bits, drop, f->n, h->d_labels, dout, dscan));
   ANNB_CUDA(cudaMemcpyAsync(labels_out, dout, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
   ANNB_CUDA(cudaStreamSynchronize(h->stream));
   return ANNB_OK;

@@ -1334,7 +1334,8 @@ int launch_filter_bitmap(annb_index *h, const uint64_t *d_filter_labels, int64_t
     mark_labels_kernel<<<(unsigned)((n_filter + 255) / 256), 256, 0, h->stream>>>(d_filter_labels, n_filter, d_by_label,
                                                                                h->max_label);
   const int64_t padded = (n + 31) / 32 * 32;
-  gather_filter_kernel<<<(unsigned)((padded + 255) / 256), 256, 0, h->stream>>>(h->d_labels, n, d_by_label, d_by_id);
+  if (n > 0)  // an empty graph has no row to gather (and a launch of 0 blocks is an error)
+    gather_filter_kernel<<<(unsigned)((padded + 255) / 256), 256, 0, h->stream>>>(h->d_labels, n, d_by_label, d_by_id);
   h->launches += 2;
   ANNB_CUDA(cudaGetLastError());
   return ANNB_OK;

@@ -274,11 +274,11 @@ ANNB_API int annb_search_wait(annb_index_t *h, int ticket);
 #define ANNB_FOP_NOTNULL 2   /* push "column col is not NULL"                                         */
 #define ANNB_FOP_INT_RANGE 3 /* INTEGER col: lo <= v <= hi, consts[a] = {int64 lo, int64 hi}         */
 #define ANNB_FOP_INT_NE 4    /* INTEGER col: v != c, consts[a] = int64 c                              */
-#define ANNB_FOP_INT_IN 5    /* INTEGER col: v in consts[a .. a + 8b), int64, sorted ascending         */
+#define ANNB_FOP_INT_IN 5    /* INTEGER col: v in consts[a .. a + 8b), int64, non-decreasing          */
 #define ANNB_FOP_INT_NIN 6   /* INTEGER col: v not in that list                                       */
 #define ANNB_FOP_FLT_RANGE 7 /* FLOAT col: lo <= v <= hi, consts[a] = {double lo, double hi}          */
 #define ANNB_FOP_FLT_NE 8    /* FLOAT col: v != c                                                     */
-#define ANNB_FOP_FLT_IN 9    /* FLOAT col: v in consts[a .. a + 8b), double, sorted ascending          */
+#define ANNB_FOP_FLT_IN 9    /* FLOAT col: v in consts[a .. a + 8b), double, non-decreasing, no NaN    */
 #define ANNB_FOP_FLT_NIN 10  /* FLOAT col: v not in that list                                         */
 #define ANNB_FOP_CODE_IN 11  /* TEXT col: bit v of the u32 bitset consts[a ..] of b bits (v >= b: 0)  */
 #define ANNB_FOP_AND 12
@@ -305,21 +305,23 @@ ANNB_API int annb_attr_set(annb_index_t *h, int col, const uint64_t *labels, int
 ANNB_API int annb_attr_export(annb_index_t *h, int col, void *values, uint8_t *valid, int64_t cap, int64_t *n_out);
 /* Drop every column (schema and values). */
 ANNB_API int annb_attr_clear(annb_index_t *h);
-/* Validate the program (op codes, columns and their types, constant ranges and alignment, stack balance and depth:
- * ANNB_EINVAL, or ANNB_ELIMIT beyond the limits above) before anything runs, bring the device columns up to date,
- * evaluate it into a bitmap the handle owns and return its id and the number of admitted rows.  One blocking call
- * per filter.  Any later change to the graph, the deletions or the attributes makes the filter stale: using it
- * then returns ANNB_ESTATE (prepare it again). */
+/* Validate the program (op codes, columns and their types, constant ranges and alignment, the order of IN / NIN lists
+ * and NaN in FLOAT ones, stack balance and depth: ANNB_EINVAL, or ANNB_ELIMIT beyond the limits above) before anything
+ * runs, bring the device columns up to date, evaluate it into a bitmap the handle owns and return its id and the
+ * number of admitted rows.  One blocking call per filter.  Any later change to the graph, the deletions or the
+ * attributes makes the filter stale: using it then returns ANNB_ESTATE (prepare it again). */
 ANNB_API int annb_filter_prepare(annb_index_t *h, const annb_filter_op_t *program, int n_ops, const void *consts,
                         int64_t n_const_bytes, int *filter_id, int64_t *count);
-/* The labels a prepared filter admits, in internal-id order (insertion order).  Writes min(cap, count) labels
- * and sets *n_out = count. */
+/* The labels of the rows a prepared filter admits, in internal-id order (insertion order): for a program, its
+ * admitted rows (*n_out = its count); for a label list, the distinct live rows the list names, so *n_out can be
+ * smaller than the list's count (repeats, labels not in the graph and deleted rows are not listed).  Writes
+ * min(cap, *n_out) labels. */
 ANNB_API int annb_filter_labels(annb_index_t *h, int filter_id, uint64_t *labels_out, int64_t cap, int64_t *n_out);
 ANNB_API int annb_filter_release(annb_index_t *h, int filter_id);
 /* A prepared filter from a label list (labels, n entries, host or device `space`): the bitmap a search with that list
  * as filter_labels would walk, made once.  Its count is n, as a label list counts (repeats and labels not in the graph
- * included), so annb_search_prepared with it returns what annb_search with the list returns.  It goes stale and is
- * released like a program-prepared filter. */
+ * included), so annb_search_prepared with it returns what annb_search with the list returns; annb_filter_labels lists
+ * the distinct live rows it names.  It goes stale and is released like a program-prepared filter. */
 ANNB_API int annb_filter_prepare_labels(annb_index_t *h, const uint64_t *labels, int64_t n, int space, int *filter_id,
                                int64_t *count);
 /* annb_search and annb_search_submit_filtered with a prepared filter in place of the label list: the bitmap is the

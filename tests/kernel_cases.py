@@ -271,19 +271,19 @@ ELSEWHERE = {
     'l2_normalize_kernel': 'tests/test_gpu_numeric_edges.py (normalised rows against the float64 rule and its switch)',
     'pack_rec0_kernel': 'tests/test_gpu_shapes.py (every search after set_graph / add_items)',
     'scatter_records_kernel': 'tests/test_gpu_build.py (incremental device-graph patches)',
-    'mark_labels_kernel': 'tests/test_gpu_walk4f.py (filter_labels -> bitmap)',
-    'gather_filter_kernel': 'tests/test_gpu_walk4f.py (filter_labels -> bitmap)',
+    'mark_labels_kernel': 'tests/test_gpu_filter_bitmaps.py (label lists -> bitmap -> listing, both sides of the sparse-label switch)',
+    'gather_filter_kernel': 'tests/test_gpu_filter_bitmaps.py (label lists -> bitmap -> listing, both sides of the sparse-label switch)',
     'export_links_kernel': 'tests/test_gpu_build_model.py (GPU builder byte for byte against the build model)',
     'link_new_nodes_kernel': 'tests/test_gpu_build_model.py (GPU builder byte for byte against the build model)',
     'reverse_link_kernel': 'tests/test_gpu_build_model.py (GPU builder byte for byte against the build model)',
     'link_new_nodes_cells_kernel': 'tests/test_gpu_build_model.py (one-pass cell-set build against the build model)',
     'reverse_link_cells_kernel': 'tests/test_gpu_build_model.py (one-pass cell-set build against the build model)',
-    'filter_eval_kernel<0>': 'tests/test_gpu_attr_filter.py (attribute filters)',
-    'filter_eval_kernel<1>': 'tests/test_gpu_attr_filter.py (attribute filters)',
+    'filter_eval_kernel<0>': 'tests/test_gpu_filter_bitmaps.py (programs against numpy at the word, grid-stride and scan edges, up to 8.4 M rows)',
+    'filter_eval_kernel<1>': 'tests/test_gpu_filter_bitmaps.py (prepare_many sets against numpy, launch splits at the LAUNCH limits)',
     'rows_copy_kernel': 'tests/test_gpu_attr_filter.py (attribute columns)',
-    'filter_compact_kernel': 'tests/test_gpu_attr_filter.py (filter_labels of a prepared filter)',
-    'filter_scan_kernel': 'tests/test_gpu_attr_filter.py (filter_labels of a prepared filter)',
-    'filter_count_kernel': 'tests/test_gpu_attr_filter.py (filter_labels of a prepared filter)',
+    'filter_compact_kernel': 'tests/test_gpu_filter_bitmaps.py (listings against numpy past the first 1 024-block chunk of the scan)',
+    'filter_scan_kernel': 'tests/test_gpu_filter_bitmaps.py (listings against numpy past the first 1 024-block chunk of the scan)',
+    'filter_count_kernel': 'tests/test_gpu_filter_bitmaps.py (listings against numpy past the first 1 024-block chunk of the scan)',
     'cell_scatter_kernel': 'tests/test_gpu_cells.py (per-cell parts of the fused cell-set walk)',
     'ivf_merge_kernel': 'tests/test_gpu_cells.py (merged cell-set rows against oracle/ivf.py)',
     'cell_probe_kernel': 'tests/test_gpu_numeric_edges.py (every adjacent pair of the probe order, float64 rule)',

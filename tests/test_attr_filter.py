@@ -9,6 +9,7 @@ import sqlite3
 import numpy as np
 import pytest
 
+import filter_cases as FC
 from conftest import GOLDEN
 from oracle.filter_eval import evaluate
 
@@ -191,6 +192,30 @@ def test_unknown_column_raises_sqlite_error():
         AttributeStore().compile({'a': {'$eq': 1}})
     with pytest.raises(ValueError, match='not supported'):
         store.compile({'a': {'$regex': 'x'}})
+
+
+def test_evaluator_matches_the_scalar_op_table():
+    """oracle.filter_eval.evaluate (numpy, what the GPU bitmaps are checked against) = a row-by-row restatement of
+    annb.h's op table on the edge-value columns and the limit programs of tests/filter_cases.py, so that a GPU
+    mismatch points at the kernel, not at the evaluator"""
+    n = 160
+    cols = FC.columns(n)
+    deleted = np.zeros(n, dtype=bool)
+    deleted[[0, 33, 64, 65, n - 1]] = True
+    # every value class is present where a program can meet it
+    assert np.isnan(cols[FC.FLOAT][0]).any() and (np.signbit(cols[FC.FLOAT][0]) & (cols[FC.FLOAT][0] == 0)).any()
+    assert {int(FC.I64.min), int(FC.I64.max)} <= set(cols[FC.INTEGER][0][cols[FC.INTEGER][1]].tolist())
+    progs = FC.programs()
+    assert {int(p['op'][0]) for _, p, _ in progs if len(p) == 1} == set(range(L.FOP_AND))
+    assert max(len(p) for _, p, _ in progs) == 255 and max(len(c) for _, _, c in progs) == L.FILTER_MAX_CONST_BYTES
+    admitted_any = 0
+    for name, program, consts in progs:
+        for dl in (None, deleted):
+            want = FC.scalar_eval(program, consts, cols, n, dl)
+            got = evaluate(program, consts, cols, n, dl)
+            assert np.array_equal(got, want), name
+        admitted_any += bool(want.any()) and not want.all()
+    assert admitted_any > len(progs) // 2          # most programs split the rows
 
 
 # ---- the library's store on a host-only handle ------------------------------------------------------------

@@ -203,12 +203,25 @@ def test_malformed_programs_are_rejected_without_a_launch(fixture_engine):
         (op(*[(L.FOP_TRUE, 0, 0, 0)] * 33 + [(L.FOP_AND, 0, 0, 0)] * 32), b'', L.ELIMIT),   # too deep
         (op(*[(L.FOP_TRUE, 0, 0, 0)] * 129 + [(L.FOP_OR, 0, 0, 0)] * 128), b'', L.ELIMIT),  # too long
         (op((L.FOP_TRUE, 0, 0, 0)), bytes(L.FILTER_MAX_CONST_BYTES + 8), L.ELIMIT),
+        # lists the evaluator's binary search cannot serve: out of order, or holding a NaN
+        (op((L.FOP_INT_IN, c_int, 0, 3)), np.array([1, 3, 2], dtype=np.int64).tobytes(), L.EINVAL),
+        (op((L.FOP_INT_NIN, c_int, 8, 2)), np.array([0, 5, -5], dtype=np.int64).tobytes(), L.EINVAL),
+        (op((L.FOP_FLT_IN, c_flt, 0, 2)), np.array([2.0, 1.0]).tobytes(), L.EINVAL),
+        (op((L.FOP_FLT_NIN, c_flt, 0, 3)), np.array([-np.inf, 0.0, -1e-300]).tobytes(), L.EINVAL),
+        (op((L.FOP_FLT_IN, c_flt, 0, 1)), np.array([np.nan]).tobytes(), L.EINVAL),
+        (op((L.FOP_FLT_NIN, c_flt, 0, 2)), np.array([1.0, np.nan]).tobytes(), L.EINVAL),
+        (op((L.FOP_TRUE, 0, 0, 0), (L.FOP_FLT_IN, c_flt, 0, 2), (L.FOP_AND, 0, 0, 0)),
+         np.array([np.nan, 1.0]).tobytes(), L.EINVAL),
     ]
     for program, consts, code in bad:
         with pytest.raises(L.AnnbError) as ei:
             e.filter_prepare(program, consts)
         assert ei.value.code == code, (program, ei.value)
     assert e.launch_count == n0
+    # equal entries are in order: -0.0 == 0.0, repeats
+    for program, consts in ((op((L.FOP_FLT_IN, c_flt, 0, 3)), np.array([-0.0, 0.0, 0.0]).tobytes()),
+                            (op((L.FOP_INT_NIN, c_int, 0, 2)), np.array([7, 7], dtype=np.int64).tobytes())):
+        e.filter_release(e.filter_prepare(program, consts)[0])
     fid, count = e.filter_prepare(op((L.FOP_TRUE, 0, 0, 0)), b'')
     assert count == N
     e.filter_release(fid)
