@@ -24,6 +24,10 @@ FILTER_MAX_PER_CALL, FILTER_LAUNCH_MAX_OPS, FILTER_LAUNCH_MAX_CONST_BYTES = 1024
  FOP_FLT_IN, FOP_FLT_NIN, FOP_CODE_IN, FOP_AND, FOP_OR) = range(14)
 # annb_filter_op_t
 FILTER_OP = np.dtype([('op', '<i4'), ('col', '<i4'), ('a', '<i4'), ('b', '<i4')])
+# annb_device_graph_export parts and header size
+GRAPH_PARTS = ('header', 'rec0', 'upper', 'labels', 'deleted', 'wide_codes', 'own_codes')
+GRAPH_MAX_LEVELS = 32
+GRAPH_HEADER_BYTES = (14 + GRAPH_MAX_LEVELS) * 8 + 128
 
 _lib = None
 
@@ -104,6 +108,7 @@ PROTOTYPES = {
     'annb_fallback_queries': (_int, [_vp, C.POINTER(_i64)]),
     'annb_sync_counts': (_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
     'annb_device_graph_layout': (_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_int)]),
+    'annb_device_graph_export': (_int, [_vp, _int, _vp, _i64, C.POINTER(_i64)]),
     'annb_set_option': (_int, [_vp, _cp, _i64]),
 }
 

@@ -290,6 +290,7 @@ struct annb_index {
   uint64_t *d_labels = nullptr;
   uint32_t *d_deleted = nullptr;
   size_t cap_rec0 = 0, cap_up = 0, cap_labels = 0, cap_deleted = 0;
+  size_t up_bytes = 0;  // bytes of d_up the last upload_upper wrote (annb_device_graph_export)
   // every node's own code (n, code_row) by internal id, for the exact subset scan; built on first use per state_gen
   uint8_t *d_own_codes = nullptr;
   size_t cap_own_codes = 0;

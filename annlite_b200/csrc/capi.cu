@@ -941,6 +941,7 @@ static int upload_upper(annb_index *h) {
   ANNB_TRY(ensure_dev((void **)&h->d_up, &h->cap_up, std::max<size_t>(up.size(), 16)));
   if (!up.empty()) ANNB_CUDA(cudaMemcpyAsync(h->d_up, up.data(), up.size(), cudaMemcpyHostToDevice, h->stream));
   d.up = h->d_up;
+  h->up_bytes = up.size();
   if (!wide) memcpy(d.ep_code, g.code(g.enterpoint), (size_t)d.code_row);  // a wide walk reads it from the code matrix
   return ANNB_OK;
 }
@@ -1060,8 +1061,16 @@ int sync_device_graph(annb_index *h) {
   d.maxlevel = g.maxlevel;
   d.ep_node = g.enterpoint;
   if (n == 0) {
+    // an emptied graph (annb_init_graph, or an empty annb_set_graph / annb_load_index): no records, and nothing of the
+    // graph it replaced stays behind -- a patch still pending from an insertion into that graph would scatter records of
+    // ids this one does not have
+    h->max_label = 0;
+    h->labels_identity = true;
+    h->up_bytes = 0;
+    h->patch_pending = false;
+    h->patch = BuildTrack();
     h->dev_dirty = false;
-    return ANNB_OK;
+    return upload_deleted(h);
   }
   if (g.maxlevel >= ANNB_MAX_LEVELS) ANNB_FAIL(ANNB_ELIMIT, "graph has %d levels (limit %d)", g.maxlevel + 1, ANNB_MAX_LEVELS);
 
@@ -1712,6 +1721,58 @@ int annb_device_graph_layout(annb_index_t *h, int64_t *rec0_bytes, int64_t *code
   if (rec0_bytes) *rec0_bytes = h->gd.rec0_bytes;
   if (code_bytes_per_node) *code_bytes_per_node = w ? wide_code_stride(h) : 0;
   if (wide) *wide = w ? 1 : 0;
+  return ANNB_OK;
+}
+
+static_assert(ANNB_GRAPH_MAX_LEVELS == ANNB_MAX_LEVELS, "annb_device_graph_export's header holds GraphDev::up_off");
+static_assert(sizeof(GraphDev::ep_code) == 128, "annb_device_graph_export's header ends with the 128 bytes of ep_code");
+
+int annb_device_graph_export(annb_index_t *h, int part, void *dst, int64_t cap, int64_t *bytes) {
+  ANNB_ENTER(h);
+  ANNB_NEED_GPU(h);
+  if (!bytes || cap < 0 || (cap > 0 && !dst)) ANNB_FAIL(ANNB_EINVAL, "null bytes / dst, or cap < 0");
+  // whatever is still walking or uploading on either lane finishes first (the copies below are synchronous)
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));
+  ANNB_CUDA(cudaStreamSynchronize(h->stream2));
+  const GraphDev &d = h->gd;
+  const int64_t n = d.n;
+  const bool wide = wide_rows(h);
+  const void *src = nullptr;  // device
+  size_t size = 0;
+  std::vector<uint8_t> head;  // host
+  switch (part) {
+    case ANNB_GRAPH_PART_HEADER: {
+      const int64_t f[14] = {d.n, d.maxlevel, d.ep_node, d.ep_rec, d.maxM, d.maxM0, d.code_row, d.rec0_bytes, d.code_off0,
+                             d.recu_bytes, d.code_offu, d.tail_offu, (int64_t)h->max_label, h->labels_identity ? 1 : 0};
+      head.resize(ANNB_GRAPH_HEADER_BYTES);
+      memcpy(head.data(), f, sizeof(f));
+      for (int l = 0; l < ANNB_MAX_LEVELS; l++) {
+        const int64_t o = (int64_t)d.up_off[l];
+        memcpy(head.data() + sizeof(f) + 8 * l, &o, 8);
+      }
+      memcpy(head.data() + sizeof(f) + 8 * ANNB_MAX_LEVELS, d.ep_code, sizeof(d.ep_code));
+      size = head.size();
+      break;
+    }
+    case ANNB_GRAPH_PART_REC0: src = d.rec0; size = d.rec0 ? (size_t)n * d.rec0_bytes : 0; break;
+    case ANNB_GRAPH_PART_UPPER: src = d.up; size = d.up ? h->up_bytes : 0; break;
+    case ANNB_GRAPH_PART_LABELS: src = d.labels; size = d.labels ? (size_t)n * 8 : 0; break;
+    case ANNB_GRAPH_PART_DELETED: src = d.deleted; size = d.deleted ? ((size_t)(n + 31) / 32 + 1) * 4 : 0; break;
+    case ANNB_GRAPH_PART_WIDE_CODES:
+      src = h->d_wide_codes;
+      size = wide && h->d_wide_codes ? (size_t)n * wide_code_stride(h) : 0;
+      break;
+    case ANNB_GRAPH_PART_OWN_CODES:
+      src = h->d_own_codes;
+      size = h->d_own_codes && h->own_codes_gen == h->state_gen ? (size_t)h->g.count.load() * h->g.code_row_bytes : 0;
+      break;
+    default: ANNB_FAIL(ANNB_EINVAL, "unknown device graph part %d", part);
+  }
+  *bytes = (int64_t)size;
+  const size_t c = std::min(size, (size_t)cap);
+  if (c == 0) return ANNB_OK;
+  if (!head.empty()) memcpy(dst, head.data(), c);
+  else ANNB_CUDA(cudaMemcpy(dst, src, c, cudaMemcpyDeviceToHost));
   return ANNB_OK;
 }
 

@@ -477,6 +477,18 @@ class Engine:
         L.check(self._lib.annb_device_graph_layout(self._h, C.byref(r), C.byref(c), C.byref(w)))
         return r.value, c.value, bool(w.value)
 
+    def device_graph_export(self, part):
+        """One part of the device walk graph (L.GRAPH_PARTS) as the last sync left it, as uint8 bytes; it does not
+        sync the graph (annb_device_graph_export documents each part's layout)."""
+        code = L.GRAPH_PARTS.index(part)
+        size = C.c_int64()
+        L.check(self._lib.annb_device_graph_export(self._h, code, None, 0, C.byref(size)))
+        out = np.zeros(max(size.value, 1), dtype=np.uint8)
+        got = C.c_int64()
+        L.check(self._lib.annb_device_graph_export(self._h, code, out.ctypes.data, size.value, C.byref(got)))
+        assert got.value == size.value
+        return out[:size.value]
+
     def set_option(self, name, value):
         L.check(self._lib.annb_set_option(self._h, name.encode(), int(value)))
 

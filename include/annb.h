@@ -509,6 +509,28 @@ ANNB_API int annb_sync_counts(annb_index_t *h, int64_t *full_syncs, int64_t *pat
  * neighbours' codes for code rows of <= 128 bytes) and the node's own code row in the by-id code matrix (wide code
  * rows only, 16-byte aligned; 0 otherwise).  *wide = 1 when the index takes the wide-row layout and hnsw_walk_wide. */
 ANNB_API int annb_device_graph_layout(annb_index_t *h, int64_t *rec0_bytes, int64_t *code_bytes_per_node, int *wide);
+/* Copies one part of the device walk graph as the last sync (search, cell-set call, GPU build) left it; diagnostics and
+ * tests only.  It does not sync the graph and runs no kernel: it waits for the handle's streams, then copies.  *bytes =
+ * the part's size; at most cap bytes are written to dst (host).  Parts:
+ *   HEADER      ANNB_GRAPH_HEADER_BYTES: int64 n, maxlevel, ep_node, ep_rec, maxM, maxM0, code_row, rec0_bytes,
+ *               code_off0, recu_bytes, code_offu, tail_offu, max_label, labels_identity, up_off[ANNB_GRAPH_MAX_LEVELS],
+ *               then the 128 bytes of ep_code
+ *   REC0        n x rec0_bytes level-0 records
+ *   UPPER       every upper level: up_off[maxlevel] + (records at maxlevel) x recu_bytes (0 when maxlevel <= 0)
+ *   LABELS      n u64 labels by internal id
+ *   DELETED     the deleted bitmap, (n + 31) / 32 + 1 u32 words (0 bytes before the first upload)
+ *   WIDE_CODES  n x up16(code_row), the by-id code matrix of wide code rows (0 bytes otherwise)
+ *   OWN_CODES   n x code_row, the own-code array of the exact subset scans when it is current (0 bytes otherwise) */
+#define ANNB_GRAPH_PART_HEADER 0
+#define ANNB_GRAPH_PART_REC0 1
+#define ANNB_GRAPH_PART_UPPER 2
+#define ANNB_GRAPH_PART_LABELS 3
+#define ANNB_GRAPH_PART_DELETED 4
+#define ANNB_GRAPH_PART_WIDE_CODES 5
+#define ANNB_GRAPH_PART_OWN_CODES 6
+#define ANNB_GRAPH_MAX_LEVELS 32
+#define ANNB_GRAPH_HEADER_BYTES ((14 + ANNB_GRAPH_MAX_LEVELS) * 8 + 128)
+ANNB_API int annb_device_graph_export(annb_index_t *h, int part, void *dst, int64_t cap, int64_t *bytes);
 /* Tuning / A-B / test switches (none changes results): "chunks" (host-buffer pipeline depth of annb_search, 1 = off),
  * "walk_kernel" (plain search: 0 hnsw_walk4 fused, 2 hnsw_walk4 over K1 tables, 1 round-1 kernels), "flagged_kernel"
  * (filter / deletions: 0 hnsw_walk4f where it applies, 1 hnsw_walk_flagged), "flagged_en" (force hnsw_walk4f's

@@ -269,8 +269,8 @@ ELSEWHERE = {
     'encode_kernel<u8>': 'tests/test_gpu_numeric_edges.py (codes against the float64 argmin rule, ties, overflow, refusals)',
     'encode_kernel<u16>': 'tests/test_gpu_numeric_edges.py (u16 codes against the float64 argmin rule, ties, overflow)',
     'l2_normalize_kernel': 'tests/test_gpu_numeric_edges.py (normalised rows against the float64 rule and its switch)',
-    'pack_rec0_kernel': 'tests/test_gpu_shapes.py (every search after set_graph / add_items)',
-    'scatter_records_kernel': 'tests/test_gpu_build.py (incremental device-graph patches)',
+    'pack_rec0_kernel': 'tests/test_gpu_device_graph.py (every full derivation, exported byte for byte against the layout model)',
+    'scatter_records_kernel': 'tests/test_gpu_device_graph.py (every patch, exported byte for byte against the layout model)',
     'mark_labels_kernel': 'tests/test_gpu_filter_bitmaps.py (label lists -> bitmap -> listing, both sides of the sparse-label switch)',
     'gather_filter_kernel': 'tests/test_gpu_filter_bitmaps.py (label lists -> bitmap -> listing, both sides of the sparse-label switch)',
     'export_links_kernel': 'tests/test_gpu_build_model.py (GPU builder byte for byte against the build model)',
