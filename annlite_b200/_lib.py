@@ -16,7 +16,7 @@ OK, EINVAL, ENODEVICE, ECUDA, ENOMEM, ESTATE, EFEWRESULTS, EIO, ECAPACITY, ENOTF
 HOST, DEVICE = 0, 1
 METRIC_L2, METRIC_IP, METRIC_COSINE = 0, 1, 2
 MAX_EF = 512
-MAX_CELLS, CELLS_GENERIC = 256, 1
+MAX_CELLS, CELLS_GENERIC, CELLS_EXACT = 256, 1, 2
 ATTR_INTEGER, ATTR_FLOAT, ATTR_TEXT = 0, 1, 2
 MAX_ATTR_COLUMNS, FILTER_MAX_OPS, FILTER_MAX_DEPTH, FILTER_MAX_CONST_BYTES = 64, 256, 32, 32768
 FILTER_MAX_PER_CALL, FILTER_LAUNCH_MAX_OPS, FILTER_LAUNCH_MAX_CONST_BYTES = 1024, 2048, 65536

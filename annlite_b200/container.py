@@ -11,6 +11,9 @@ Differences from the reference, besides the docarray / SQLite / RocksDB stores i
   `bruteforce_filter_below`, read on every call, is passed along: a filter that admits at most that many of the cell's
   rows is scanned exactly inside the same GPU search, as the cell's own search_batch would scan it.  Unfiltered
   searches after deletions search the cells one by one.
+* `exact=True` (search_cells, ivf_search) is IVF-PQ with exact ADC top-k inside the probed cells: every probed cell is
+  scanned exactly over its live rows, or over the rows the filter admits there, in the same one GPU search, and no
+  graph is walked.  Results are exact by construction; n_probe trades recall for speed.
 * equal distances in the merge keep concatenation order (the reference's argsort leaves them unspecified); a query
   with fewer than `limit` results is padded with +inf / UINT64_MAX / cell -1.
 * with a VQCodec attached, cells are probed in the order of annlite.math.cdist over the centroids.  The reference's
@@ -175,24 +178,29 @@ class CellContainer:
             self._live[c] -= 1
 
     # ---- search (container.py:88-144, 201-260) ---------------------------------------------------------
-    def ivf_search(self, x: 'np.ndarray', cells: 'np.ndarray', filter=None, limit: int = 10):
-        """One query over `cells` in the given order -> (dists (limit,), ids (limit,), cell_ids (limit,))."""
+    def ivf_search(self, x: 'np.ndarray', cells: 'np.ndarray', filter=None, limit: int = 10, exact: bool = False):
+        """One query over `cells` in the given order -> (dists (limit,), ids (limit,), cell_ids (limit,)).  `exact` as
+        in search_cells."""
         x = np.ascontiguousarray(x, dtype=np.float32).reshape(1, -1)
-        d, i, c = self._search_cells(x, np.asarray(cells, dtype=np.int32).reshape(1, -1), filter=filter, limit=limit)
+        d, i, c = self._search_cells(x, np.asarray(cells, dtype=np.int32).reshape(1, -1), filter=filter, limit=limit,
+                                     exact=exact)
         return d[0], i[0], c[0]
 
-    def search_cells(self, query: 'np.ndarray', cells=None, filter=None, limit: int = 10):
+    def search_cells(self, query: 'np.ndarray', cells=None, filter=None, limit: int = 10, exact: bool = False):
         """A batch -> (dists (B, limit), ids (B, limit), cell_ids (B, limit)).  `cells` = (B, n_probe) probe order, or
         None: every cell, nearest VQ centroid first (AnnLite._cell_selection with n_probe = n_cells,
-        annlite/index.py:94, :458-466), computed on the GPU."""
-        return self._search_cells(np.ascontiguousarray(query, dtype=np.float32), cells, filter=filter, limit=limit)
+        annlite/index.py:94, :458-466), computed on the GPU.  `exact` = scan every probed cell exactly instead of
+        walking its graph: each cell's part is the exact ADC top-k of its live rows (or of the rows the filter admits
+        there), in one GPU search."""
+        return self._search_cells(np.ascontiguousarray(query, dtype=np.float32), cells, filter=filter, limit=limit,
+                                  exact=exact)
 
     def probe_order(self, query: 'np.ndarray', n_probe: Optional[int] = None):
         if self.vq_codec is None:
             raise ValueError('no VQCodec attached: pass the cells to search')
         return self._cells().probe(np.ascontiguousarray(query, dtype=np.float32), n_probe)
 
-    def _search_cells(self, x, cells=None, filter=None, limit: int = 10, generic=False):
+    def _search_cells(self, x, cells=None, filter=None, limit: int = 10, generic=False, exact=False):
         if x.ndim == 1:
             x = x.reshape(1, -1)
         B = x.shape[0]
@@ -205,15 +213,15 @@ class CellContainer:
         v0 = self._vec_indexes[0]
         if filter is None or (isinstance(filter, dict) and not filter):
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
-                                       generic=generic)
+                                       generic=generic, exact=exact)
             return dist, lab, cid
         per_query = is_per_query_filter(filter)
         if per_query and len(filter) != B:
             raise ValueError(f'{len(filter)} filters for {B} queries')
-        if not generic:
+        if not generic or exact:   # (exact with generic: the same scans, one launch per cell)
             if per_query:
-                return self._search_cells_multi(x, cells, filter, limit)
-            return self._search_cells_prepared(x, cells, filter, limit)
+                return self._search_cells_multi(x, cells, filter, limit, generic=generic, exact=exact)
+            return self._search_cells_prepared(x, cells, filter, limit, generic=generic, exact=exact)
         # filtered, per-cell route: one filtered search per probed cell (HnswIndex.search_batch shrinks the limit to
         # what the filter admits there, hnsw/index.py:151-154), then the same merge on the GPU
         lab = np.full((B, self.n_cells, limit), _NONE, dtype=np.uint64)
@@ -259,7 +267,7 @@ class CellContainer:
             return None
         return np.array([-1 if b is None else int(b) for b in below], dtype=np.int64)
 
-    def _search_cells_prepared(self, x, cells, filter, limit):
+    def _search_cells_prepared(self, x, cells, filter, limit, generic=False, exact=False):
         """A dict filter or an id array over the probed cells in one GPU search (annb_cellset_search_prepared): the
         filter is prepared on each probed cell (an id array split by cell, each share prepared as a label list), and
         every cell's k is what the per-cell route's search_batch uses: min(limit, live rows, admitted count).  A cell
@@ -288,13 +296,14 @@ class CellContainer:
                     prepared.append(PreparedFilter(e, *e.filter_prepare_labels(mine.astype(np.uint64))))
                 fids[c] = prepared[-1].id
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
-                                       filter_ids=fids, bruteforce_below=self._bruteforce_below())
+                                       filter_ids=fids, bruteforce_below=self._bruteforce_below(), generic=generic,
+                                       exact=exact)
         finally:
             for p in prepared:
                 p.release()
         return dist, lab, cid
 
-    def _search_cells_multi(self, x, cells, filters, limit):
+    def _search_cells_multi(self, x, cells, filters, limit, generic=False, exact=False):
         """One filter dict per query over the probed cells in one GPU search (annb_cellset_search_multi): the list is
         prepared on each probed cell with rows (HnswIndex.prepare_filters), whose ids form that cell's column of the
         (B, n_cells) table; every pair's k is what the per-cell route's search_batch uses: min(limit, live rows,
@@ -312,7 +321,8 @@ class CellContainer:
                 prepared.append(self._vec_indexes[c].prepare_filters(filters))
                 qids[:, c] = prepared[-1].ids
             lab, dist, cid = cs.search(x, limit=limit, ef=v0.ef_search, normalize=v0._normalize_rounds, order=cells,
-                                       query_filter_ids=qids, bruteforce_below=self._bruteforce_below())
+                                       query_filter_ids=qids, bruteforce_below=self._bruteforce_below(), generic=generic,
+                                       exact=exact)
         finally:
             for p in prepared:
                 p.release()

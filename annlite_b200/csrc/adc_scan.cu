@@ -629,20 +629,33 @@ int launch_merge_topk(annb_index *h, const uint64_t *labels, const float *dists,
   return ANNB_OK;
 }
 
-// ---- the multi-subset exact scan (annb_cellset_search_prepared / _multi with bruteforce thresholds) -------------
-// A job is one subset of one cell (a prepared filter's admitted rows, or a label list's live entries) and the query rows
-// that scan it.  Gather: every job's subset is compacted (bitmap, in internal-id order, as annb_filter_labels lists it)
-// or read (id list, in order, repeats kept), and its code rows and labels are copied once from the cell's own-code array
-// into a contiguous scratch -- three launches for all jobs.  Scan: one launch for all jobs, a CTA per tile of one job's
-// queries.  k <= 16: scan_topk_tiled2's mapping (16 interleaved tables, a half-warp scores one row for 16 queries,
-// per-lane register lists, one CTA reduction); larger k: a warp per query with its table in shared memory and a
-// WarpList, as scan_topk_kernel.  The subset is never chunked, so each CTA's lists are final and go straight to the
-// pair's row of the by-cell scratch.  Arithmetic and order are K2's: d = sum_m T[m, code[m]] from 0.f in fp32, the k
-// best by (distance, position in the subset) -- annb_scan_subset's bits and order.
+// ---- the multi-subset exact scan (annb_cellset_search* with bruteforce thresholds or ANNB_CELLS_EXACT) --------
+// A job is one subset of one cell (a prepared filter's admitted rows, a label list's live entries, or the cell's live
+// rows) and the query rows that scan it.  Gather: every job's subset is compacted (bitmap, in internal-id order, as
+// annb_filter_labels lists it; the live rows through the deletion bitmap read inverted) or read (id list, in order,
+// repeats kept), and its code rows and labels are copied once from the cell's own-code array into a contiguous scratch
+// -- three launches for all jobs; a cell without deletions is scanned in place.  Scan: one launch for all jobs, a CTA
+// per tile of one job's queries.  k <= 16: scan_topk_tiled2's mapping (16 interleaved tables, a half-warp scores one
+// row for 16 queries, per-lane register lists, one CTA reduction); larger k: a warp per query with its table in shared
+// memory and a WarpList, as scan_topk_kernel.  Unchunked, each CTA's lists are final and go straight to the pair's row
+// of the by-cell scratch.  When the tiles are too few to fill the GPU (subset_scan_chunk_rows), each tile is split
+// into row chunks, one CTA each; the last CTA of a tile to finish merges its chunks' lists in the same launch.
+// Arithmetic and order are K2's: d = sum_m T[m, code[m]] from 0.f in fp32, the k best by (distance, position in the
+// subset) -- annb_scan_subset's bits and order, chunked or not.
 namespace {
 
 constexpr int GATHER_THREADS = 256;  // one bitmap word (or one list entry) per thread
 constexpr int SCAN_WARP_TILE = 8;    // queries per CTA of the warp-per-query form
+constexpr int SUBSET_MAX_CHUNKS = 16;       // a tile's chunk lists are merged by one lane each
+constexpr int64_t SUBSET_MIN_CHUNK = 4096;  // rows: a chunk amortises staging its CTA's tables (128 KB for 16 queries)
+
+// word w of a job's bitmap as it admits rows: a filter's as it is, the deletions (SUBSET_LIVE) inverted over the cell's rows
+__device__ __forceinline__ uint32_t subset_word(const SubsetScan &J, int64_t w) {
+  const uint32_t x = J.bits[w];
+  if (J.kind != SUBSET_LIVE) return x;
+  const int64_t valid = J.n_rows - w * 32;
+  return ~x & (valid >= 32 ? 0xffffffffu : ((1u << valid) - 1u));
+}
 
 // pass 1: admitted rows per block of a job's bitmap
 __global__ void __launch_bounds__(GATHER_THREADS) subset_count_kernel(const SubsetScan *__restrict__ jobs) {
@@ -654,7 +667,7 @@ __global__ void __launch_bounds__(GATHER_THREADS) subset_count_kernel(const Subs
   if (threadIdx.x == 0) s = 0;
   __syncthreads();
   const int64_t w = (int64_t)blockIdx.x * GATHER_THREADS + threadIdx.x;
-  unsigned int c = w < J.nwords ? __popc(J.bits[w]) : 0u;
+  unsigned int c = w < J.nwords ? __popc(subset_word(J, w)) : 0u;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL_MASK, c, o);
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s, c);
@@ -681,7 +694,7 @@ __global__ void __launch_bounds__(GATHER_THREADS) subset_gather_kernel(const Sub
   const SubsetScan &J = jobs[blockIdx.y];
   const int64_t t = (int64_t)blockIdx.x * GATHER_THREADS + threadIdx.x;
   if (!J.bits) {
-    if (blockIdx.x * (int64_t)GATHER_THREADS >= J.n) return;
+    if (!J.ids || blockIdx.x * (int64_t)GATHER_THREADS >= J.n) return;  // (a live-rows job without deletions: in place)
     if (t < J.n) {
       const uint32_t id = J.ids[t];
       reinterpret_cast<uint2 *>(J.codes)[t] = __ldg(reinterpret_cast<const uint2 *>(J.cell_codes) + id);
@@ -692,7 +705,7 @@ __global__ void __launch_bounds__(GATHER_THREADS) subset_gather_kernel(const Sub
   if (blockIdx.x * (int64_t)GATHER_THREADS >= J.nwords) return;
   __shared__ unsigned int warp_sums[GATHER_THREADS / 32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  uint32_t word = t < J.nwords ? J.bits[t] : 0u;
+  uint32_t word = t < J.nwords ? subset_word(J, t) : 0u;
   const unsigned int c = __popc(word);
   unsigned int x = c;  // inclusive scan over the warp, then over the warps
 #pragma unroll
@@ -726,20 +739,80 @@ __device__ __forceinline__ void subset_write_tail(const SubsetScan &J, int64_t r
   }
 }
 
+// this CTA's chunk lists are written: true in the tile's last CTA to finish (which then reads every chunk's lists)
+__device__ __forceinline__ bool subset_last_chunk(const SubsetScan &J, const SubsetChunks &ch, int group) {
+  __shared__ int last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned int nch = (unsigned int)((J.n + ch.rows - 1) / ch.rows);
+    last = atomicAdd(ch.done + group, 1u) == nch - 1;
+  }
+  __syncthreads();
+  if (last) __threadfence();
+  return last;
+}
+
+// a query's chunk lists (list0 = its first; one per chunk of the subset, each K sorted (distance, position) entries)
+// merged by one warp into the pair's row: lane l walks list l, and each step takes the smallest head by (distance,
+// position) -- the unchunked scan's k best exactly
+__device__ __forceinline__ void subset_merge_chunks(const SubsetScan &J, const SubsetChunks &ch, int64_t list0, int64_t row, int limit,
+                                    uint64_t *__restrict__ sl, float *__restrict__ sd, int32_t *__restrict__ sfound,
+                                    int64_t *__restrict__ sstats) {
+  const int lane = threadIdx.x & 31;
+  const int nch = (int)((J.n + ch.rows - 1) / ch.rows);
+  const int64_t base = (list0 + lane) * ch.K;
+  int h = 0;
+  float d = CUDART_INF_F;
+  uint32_t id = LIST_EMPTY_VAL;
+  if (lane < nch) {
+    d = __ldcg(ch.part_d + base);
+    id = __ldcg(ch.part_i + base);
+  }
+  for (int j = 0; j < J.k; j++) {
+    float md = d;
+    uint32_t mi = id;
+#pragma unroll
+    for (int s2 = 16; s2 > 0; s2 >>= 1) {
+      const float od = __shfl_xor_sync(FULL_MASK, md, s2);
+      const uint32_t oi = __shfl_xor_sync(FULL_MASK, mi, s2);
+      if (od < md || (od == md && oi < mi)) {
+        md = od;
+        mi = oi;
+      }
+    }
+    if (lane == 0) {
+      sd[row * limit + j] = md;
+      sl[row * limit + j] = mi == LIST_EMPTY_VAL ? UINT64_MAX : J.labels[mi];
+    }
+    if (id == mi && mi != LIST_EMPTY_VAL) {  // positions are unique across the chunks: exactly one lane advances
+      if (++h < ch.K) {
+        d = __ldcg(ch.part_d + base + h);
+        id = __ldcg(ch.part_i + base + h);
+      } else {
+        d = CUDART_INF_F;
+        id = LIST_EMPTY_VAL;
+      }
+    }
+  }
+  if (lane == 0) subset_write_tail(J, row, sfound, sstats);
+}
+
 // tile i = (job, first query of the job); 16 queries per CTA, 16 warps
 template <int KK>
 __global__ void __launch_bounds__(TILED_WARPS * 32, 1)
-subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__restrict__ jobs, const int2 *__restrict__ tiles,
-                         int n_cells, int limit, uint64_t *__restrict__ sl, float *__restrict__ sd, int32_t *__restrict__ sfound,
-                         int64_t *__restrict__ sstats) {
+subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__restrict__ jobs, const int4 *__restrict__ tiles,
+                         const SubsetChunks ch, int n_cells, int limit, uint64_t *__restrict__ sl, float *__restrict__ sd,
+                         int32_t *__restrict__ sfound, int64_t *__restrict__ sstats) {
   constexpr int M = 8, KS = 256, TS = M * KS;
   extern __shared__ float sT[];
   __shared__ int64_t srow[QT];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int half = lane >> 4, q = lane & 15;
-  const int2 tile = tiles[blockIdx.x];
+  const int4 tile = tiles[blockIdx.x];
   const SubsetScan &J = jobs[tile.x];
   const int q0 = tile.y, nq = min(QT, J.nq - q0);
+  const bool chunked = ch.rows > 0;
   if (threadIdx.x < QT) srow[threadIdx.x] = threadIdx.x < nq ? (int64_t)J.queries[q0 + threadIdx.x] : -1;
   __syncthreads();
   for (int t = threadIdx.x; t < TS * QT; t += blockDim.x) {
@@ -754,7 +827,8 @@ subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__r
     Kd[i] = CUDART_INF_F;
     Ki[i] = LIST_EMPTY_VAL;
   }
-  const int64_t n = J.n;
+  const int64_t r0 = chunked ? (int64_t)tile.z * ch.rows : 0;
+  const int64_t n = chunked ? min(J.n, r0 + ch.rows) : J.n;  // rows [r0, n) of the subset
   const uint8_t *codes = J.codes;
   const float *Tq = sT + q;
   auto score = [&](const uint2 c) -> float {  // m sequential from 0.f, every add rounded (pq_bindings.pyx:30-47)
@@ -770,7 +844,7 @@ subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__r
     return d;
   };
   constexpr int64_t STEP = 2 * TILED_WARPS;
-  int64_t r = 2 * warp + half;
+  int64_t r = r0 + 2 * warp + half;
   for (; r + STEP < n; r += 2 * STEP) {
     const uint2 ca = __ldg(reinterpret_cast<const uint2 *>(codes + r * 8));
     const uint2 cb = __ldg(reinterpret_cast<const uint2 *>(codes + (r + STEP) * 8));
@@ -807,9 +881,10 @@ subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__r
     Kd[i] = half == 0 ? rd[(warp * TILED_WARPS + q) * KK + i] : CUDART_INF_F;
     Ki[i] = half == 0 ? ri[(warp * TILED_WARPS + q) * KK + i] : LIST_EMPTY_VAL;
   }
-  if (warp >= nq) return;
+  // warp w < nq: the k best of query w's list -> its pair's row, or (chunked) the K best -> its chunk list
   const int64_t row = srow[warp] * n_cells + J.cell;
-  const int k = J.k;
+  const int64_t list0 = ((int64_t)tile.w * QT + warp) * ch.G;
+  const int k = warp >= nq ? 0 : (chunked ? ch.K : J.k);
   for (int j = 0; j < k; j++) {
     float md = Kd[0];
     uint32_t mi = Ki[0];
@@ -822,7 +897,10 @@ subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__r
         mi = oi;
       }
     }
-    if (lane == 0) {
+    if (lane == 0 && chunked) {
+      ch.part_d[(list0 + tile.z) * ch.K + j] = md;
+      ch.part_i[(list0 + tile.z) * ch.K + j] = mi;
+    } else if (lane == 0) {
       sd[row * limit + j] = md;
       sl[row * limit + j] = mi == LIST_EMPTY_VAL ? UINT64_MAX : J.labels[mi];
     }
@@ -836,32 +914,39 @@ subset_scan_tiled_kernel(const float *__restrict__ tables, const SubsetScan *__r
       Ki[KK - 1] = LIST_EMPTY_VAL;
     }
   }
-  if (lane == 0) subset_write_tail(J, row, sfound, sstats);
+  if (!chunked) {
+    if (lane == 0 && warp < nq) subset_write_tail(J, row, sfound, sstats);
+    return;
+  }
+  if (subset_last_chunk(J, ch, tile.w) && warp < nq) subset_merge_chunks(J, ch, list0, row, limit, sl, sd, sfound, sstats);
 }
 
 // k > 16: a warp per query (SCAN_WARP_TILE queries of one job per CTA), its table in shared memory, lanes over rows
 template <int EPL>
 __global__ void __launch_bounds__(SCAN_WARP_TILE * 32)
-subset_scan_warp_kernel(const float *__restrict__ tables, const SubsetScan *__restrict__ jobs, const int2 *__restrict__ tiles,
-                        int n_cells, int limit, uint64_t *__restrict__ sl, float *__restrict__ sd, int32_t *__restrict__ sfound,
-                        int64_t *__restrict__ sstats) {
+subset_scan_warp_kernel(const float *__restrict__ tables, const SubsetScan *__restrict__ jobs, const int4 *__restrict__ tiles,
+                        const SubsetChunks ch, int n_cells, int limit, uint64_t *__restrict__ sl, float *__restrict__ sd,
+                        int32_t *__restrict__ sfound, int64_t *__restrict__ sstats) {
   constexpr int TS = 8 * 256;
   extern __shared__ float sT[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int2 tile = tiles[blockIdx.x];
+  const int4 tile = tiles[blockIdx.x];
   const SubsetScan &J = jobs[tile.x];
   const int qi = tile.y + warp;
-  if (qi >= J.nq) return;
-  const int64_t qrow = J.queries[qi];
+  const bool chunked = ch.rows > 0;
+  if (qi >= J.nq && !chunked) return;  // (chunked: every warp takes part in the CTA's hand-over)
+  const bool active = qi < J.nq;
+  const int64_t qrow = active ? J.queries[qi] : 0;
   float *T = sT + warp * TS;
   for (int i = lane; i < TS; i += 32) T[i] = __ldg(tables + qrow * TS + i);
   __syncwarp();
-  const int k = J.k;
-  const int64_t n = J.n;
+  const int k = chunked ? ch.K : J.k;
+  const int64_t r0 = chunked ? (int64_t)tile.z * ch.rows : 0;
+  const int64_t n = !active ? 0 : (chunked ? min(J.n, r0 + ch.rows) : J.n);  // rows [r0, n) of the subset
   WarpList<EPL> L;
   L.clear();
   float worst = CUDART_INF_F;
-  for (int64_t base = 0; base < n; base += 32) {
+  for (int64_t base = r0; base < n; base += 32) {
     const int64_t r = base + lane;
     float d = CUDART_INF_F;
     if (r < n) d = adc_lookup_u8x8(T, __ldg(reinterpret_cast<const uint2 *>(J.codes) + r), 256);
@@ -877,15 +962,30 @@ subset_scan_warp_kernel(const float *__restrict__ tables, const SubsetScan *__re
     }
   }
   const int64_t row = qrow * n_cells + J.cell;
+  if (!chunked) {
 #pragma unroll
-  for (int e = 0; e < EPL; e++) {
-    const int pos = e * 32 + lane;
-    if (pos < k) {
-      sd[row * limit + pos] = L.k[e];
-      sl[row * limit + pos] = L.v[e] == LIST_EMPTY_VAL ? UINT64_MAX : J.labels[L.v[e]];
+    for (int e = 0; e < EPL; e++) {
+      const int pos = e * 32 + lane;
+      if (pos < k) {
+        sd[row * limit + pos] = L.k[e];
+        sl[row * limit + pos] = L.v[e] == LIST_EMPTY_VAL ? UINT64_MAX : J.labels[L.v[e]];
+      }
+    }
+    if (lane == 0) subset_write_tail(J, row, sfound, sstats);
+    return;
+  }
+  const int64_t list0 = ((int64_t)tile.w * SCAN_WARP_TILE + warp) * ch.G;
+  if (active) {
+#pragma unroll
+    for (int e = 0; e < EPL; e++) {
+      const int pos = e * 32 + lane;
+      if (pos < k) {
+        ch.part_d[(list0 + tile.z) * ch.K + pos] = L.k[e];
+        ch.part_i[(list0 + tile.z) * ch.K + pos] = L.v[e];
+      }
     }
   }
-  if (lane == 0) subset_write_tail(J, row, sfound, sstats);
+  if (subset_last_chunk(J, ch, tile.w) && active) subset_merge_chunks(J, ch, list0, row, limit, sl, sd, sfound, sstats);
 }
 
 }  // namespace
@@ -894,37 +994,62 @@ bool subset_scan_applicable(const annb_index *h) { return h->M == 8 && h->code_b
 
 int subset_scan_tile_width(int kmax) { return kmax <= 16 ? QT : SCAN_WARP_TILE; }
 
+// Unchunked while the tiles alone make two waves of CTAs (the tiled form holds one CTA per SM): every CTA's lists are
+// then final, with no hand-over.  Fewer tiles -- a small batch over large subsets, such as whole cells -- are cut into
+// chunks of at least SUBSET_MIN_CHUNK rows, at most SUBSET_MAX_CHUNKS per subset, enough for about two waves.
+int64_t subset_scan_chunk_rows(const annb_index *h, int64_t tiles, int64_t longest) {
+  const int64_t floor_rows = (longest + SUBSET_MAX_CHUNKS - 1) / SUBSET_MAX_CHUNKS;
+  int64_t rows;
+  if (h->opt_subset_chunk_rows != 0) {
+    if (h->opt_subset_chunk_rows < 0) return 0;
+    rows = std::max(h->opt_subset_chunk_rows, floor_rows);
+  } else {
+    const int64_t target = 2LL * h->sm_count;
+    if (tiles <= 0 || tiles >= target) return 0;
+    const int64_t g = std::min<int64_t>(SUBSET_MAX_CHUNKS, (target + tiles - 1) / tiles);
+    rows = std::max<int64_t>(SUBSET_MIN_CHUNK, (longest + g - 1) / g);
+    rows = (rows + 31) / 32 * 32;
+  }
+  return longest > rows ? rows : 0;
+}
+
 int launch_subset_scan(annb_index *h, cudaStream_t st, const SubsetScan *d_jobs, const std::vector<SubsetScan> &jobs,
-                       const int2 *d_tiles, int64_t n_tiles, const float *tables, int n_cells, int limit, uint64_t *sl,
-                       float *sd, int32_t *sfound, int64_t *sstats) {
+                       const int4 *d_tiles, int64_t n_tiles, const SubsetChunks &ch, const float *tables, int n_cells, int limit,
+                       uint64_t *sl, float *sd, int32_t *sfound, int64_t *sstats) {
   const int J = (int)jobs.size();
   if (J == 0 || n_tiles == 0) return ANNB_OK;
   if (J > 65535) ANNB_FAIL(ANNB_ELIMIT, "%d subsets in one scan (limit 65535)", J);
   int64_t gx = 1;
   int kmax = 1;
   bool any_bits = false;
+  bool any_gather = false;
   for (const SubsetScan &s : jobs) {
     gx = std::max(gx, s.bits ? (s.nwords + GATHER_THREADS - 1) / GATHER_THREADS : (s.n + GATHER_THREADS - 1) / GATHER_THREADS);
     kmax = std::max(kmax, (int)s.k);
     any_bits |= s.bits != nullptr;
+    any_gather |= s.bits != nullptr || s.ids != nullptr;
   }
   if (kmax > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "k=%d exceeds ANNB_MAX_EF=%d", kmax, ANNB_MAX_EF);
+  if (ch.rows > 0 && (ch.K < kmax || ch.G > SUBSET_MAX_CHUNKS))
+    ANNB_FAIL(ANNB_ESTATE, "internal: chunk lists of %d entries / %d chunks for k=%d", ch.K, ch.G, kmax);
   const dim3 ggrid((unsigned)gx, (unsigned)J);
   if (any_bits) {
     subset_count_kernel<<<ggrid, GATHER_THREADS, 0, st>>>(d_jobs);
     subset_offsets_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_jobs, J);
     h->launches += 2;
   }
-  subset_gather_kernel<<<ggrid, GATHER_THREADS, 0, st>>>(d_jobs);
-  h->launches++;
-  ANNB_CUDA(cudaGetLastError());
+  if (any_gather) {
+    subset_gather_kernel<<<ggrid, GATHER_THREADS, 0, st>>>(d_jobs);
+    h->launches++;
+    ANNB_CUDA(cudaGetLastError());
+  }
   if (kmax <= 16) {
     const size_t smem = (size_t)8 * 256 * QT * sizeof(float);
 #define SS_TILED(KKV)                                                                                                    \
   {                                                                                                                      \
     ANNB_CUDA(cudaFuncSetAttribute(subset_scan_tiled_kernel<KKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    subset_scan_tiled_kernel<KKV><<<(unsigned)n_tiles, TILED_WARPS * 32, smem, st>>>(tables, d_jobs, d_tiles, n_cells, limit, sl, sd, \
-                                                                                   sfound, sstats);                    \
+    subset_scan_tiled_kernel<KKV><<<(unsigned)n_tiles, TILED_WARPS * 32, smem, st>>>(tables, d_jobs, d_tiles, ch, n_cells, limit, sl, \
+                                                                                   sd, sfound, sstats);                \
   }
     if (kmax <= 1) SS_TILED(1)
     else if (kmax <= 10) SS_TILED(10)
@@ -935,8 +1060,8 @@ int launch_subset_scan(annb_index *h, cudaStream_t st, const SubsetScan *d_jobs,
 #define SS_WARP(E)                                                                                                       \
   {                                                                                                                      \
     ANNB_CUDA(cudaFuncSetAttribute(subset_scan_warp_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    subset_scan_warp_kernel<E><<<(unsigned)n_tiles, SCAN_WARP_TILE * 32, smem, st>>>(tables, d_jobs, d_tiles, n_cells, limit, sl, sd, \
-                                                                                   sfound, sstats);                    \
+    subset_scan_warp_kernel<E><<<(unsigned)n_tiles, SCAN_WARP_TILE * 32, smem, st>>>(tables, d_jobs, d_tiles, ch, n_cells, limit, sl, \
+                                                                                   sd, sfound, sstats);                \
   }
     const int epl = (kmax + 31) / 32;
     if (epl <= 1) SS_WARP(1)

@@ -214,10 +214,15 @@ struct PreparedFilter {
 // subset is a bitmap by internal id, compacted in id order (the order annb_filter_labels lists it), or a list of
 // internal ids; its code rows and labels are gathered once into `codes` / `labels`.  Each query row in `queries` gets
 // the k best (distance, position in the subset) in its pair's row (q * n_cells + cell) of the by-cell scratch.
+// Kind SUBSET_LIVE is a cell's live rows in id order: its deletion bitmap read inverted (`bits`, over n_rows ids), or
+// with no deletions (bits == nullptr) every row, scanned in place (codes / labels are the cell's own arrays, nothing is
+// gathered).
+enum { SUBSET_FILTER = 0, SUBSET_LIVE = 1 };
 struct SubsetScan {
   const uint32_t *bits;        // bitmap by internal id, or nullptr
-  const uint32_t *ids;         // when bits == nullptr: internal ids in order
+  const uint32_t *ids;         // SUBSET_FILTER with bits == nullptr: internal ids in order
   int64_t nwords;              // bitmap words to compact
+  int64_t n_rows;              // SUBSET_LIVE: the cell's rows (ids 0..n_rows-1)
   const uint8_t *cell_codes;   // the cell's (rows, 8) own codes by internal id
   const uint64_t *cell_labels; // the cell's labels by internal id
   uint8_t *codes;              // gathered (n, 8) code rows
@@ -225,7 +230,18 @@ struct SubsetScan {
   unsigned int *block_offs;    // bitmap: per-block counts, then offsets
   int64_t n;                   // subset rows
   const uint32_t *queries;     // query rows that scan the subset
-  int32_t nq, k, cell, pad;
+  int32_t nq, k, cell, kind;
+};
+
+// Row chunks of one multi-subset scan launch.  rows == 0: each tile's CTA scans its subset whole.  rows > 0: a tile
+// (job, first query) becomes one CTA per chunk of `rows` rows; each writes its queries' K best of the chunk (K = the
+// launch's largest k) to a list, and the last of the tile's CTAs to finish merges those lists into the pairs' rows.
+struct SubsetChunks {
+  int64_t rows;
+  int G, K;                    // the most chunks of any subset; entries per list
+  float *part_d;               // (tile groups, tile width, G, K)
+  uint32_t *part_i;
+  unsigned int *done;          // (tile groups) chunk CTAs finished, zeroed before the launch
 };
 
 // An enqueued search batch, as its flagged queries (found = -1) are re-run on the bitmap walk (capi.cu: rerun_flagged).
@@ -331,6 +347,7 @@ struct annb_index {
   int64_t opt_walk_kernel = 0;     // plain search: 0 = hnsw_walk4 with fused K1 (default), 1 = round-1 kernels (K1 +
                                    // hnsw_walk_fast), 2 = hnsw_walk4 over materialised tables (K1 + TMA staging)
   int64_t opt_scan_kernel = 0;     // K2 scan + top-k: 0 = query-tiled kernel where it applies, 1 = round-1 kernel, 2 = tiled even for small inputs (tests), 3 = first tiled version, forced
+  int64_t opt_subset_chunk_rows = 0;  // multi-subset scan: 0 = chunked by its size rule, -1 = never, > 0 = chunks of this many rows
   int64_t opt_gpu_build = 1;       // add_items with num_threads != 1 and >= 16384 fresh rows: level-0 insertion on the GPU
   int64_t opt_gpu_build_frac = 16; // a GPU-built batch is at most 1/frac of the graph it is inserted into
   int64_t reserve_nodes = 0;       // sync_device_graph sizes the device graph for this many nodes (GPU builder)
@@ -422,9 +439,12 @@ int sync_own_codes(annb_index *h, const uint8_t **out);
 // results straight into the by-cell scratch (found = k, counters {0, 0, n}); M = 8 one-byte codes, Ks = 256 only
 bool subset_scan_applicable(const annb_index *h);
 int subset_scan_tile_width(int kmax);
+// rows per chunk of a launch whose unchunked form has `tiles` CTAs and whose longest subset has `longest` rows (0 =
+// unchunked); tiles are int4 {job, first query, chunk, tile group}
+int64_t subset_scan_chunk_rows(const annb_index *h, int64_t tiles, int64_t longest);
 int launch_subset_scan(annb_index *h, cudaStream_t st, const SubsetScan *d_jobs, const std::vector<SubsetScan> &jobs,
-                       const int2 *d_tiles, int64_t n_tiles, const float *tables, int n_cells, int limit, uint64_t *sl,
-                       float *sd, int32_t *sfound, int64_t *sstats);
+                       const int4 *d_tiles, int64_t n_tiles, const SubsetChunks &ch, const float *tables, int n_cells, int limit,
+                       uint64_t *sl, float *sd, int32_t *sfound, int64_t *sstats);
 // G ascending (dist, label) lists of k per query -> global k best; *_gstride = distance between two shards' arrays in elements
 int launch_merge_topk(annb_index *h, const uint64_t *labels, const float *dists, int G, int64_t B, int k, int64_t l_gstride,
                       int64_t d_gstride, uint64_t *labels_out, float *dists_out, cudaStream_t stream);

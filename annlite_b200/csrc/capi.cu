@@ -1795,6 +1795,7 @@ int annb_set_option(annb_index_t *h, const char *name, int64_t value) {
   else if (!strcmp(name, "flagged_kernel")) h->opt_flagged_kernel = value;
   else if (!strcmp(name, "flagged_en")) h->opt_flagged_en = value;
   else if (!strcmp(name, "scan_kernel")) h->opt_scan_kernel = value;
+  else if (!strcmp(name, "subset_chunk_rows")) h->opt_subset_chunk_rows = value;
   else if (!strcmp(name, "walk_kernel")) h->opt_walk_kernel = value;
   else if (!strcmp(name, "dump_tables")) h->opt_dump_tables = value;
   else if (!strcmp(name, "gpu_build")) h->opt_gpu_build = value;

@@ -21,15 +21,15 @@ struct annb_cellset {
   annb_index *h0 = nullptr;         // its stream and scratch serve the cell set's launches
   float *d_centroids = nullptr;     // (n_cells, dim) or nullptr (then every search needs an explicit order)
   GraphDev *d_graphs = nullptr;     // (n_cells) descriptors, re-read before every fused search
-  void *buf[24] = {nullptr};
-  size_t cap[24] = {0};
+  void *buf[26] = {nullptr};
+  size_t cap[26] = {0};
   float probe_ms = 0, walk_ms = 0, merge_ms = 0;
   cudaEvent_t ev[8] = {nullptr};    // [0,1] probe, [2,3] walk, [4,5] merge, [6,7] hand-over to a cell's stream and back
   int last_route = 0;
   int64_t last_rerun_pairs = 0;     // annb_cellset_search_prepared / _multi: (query, cell) pairs re-run on the bitmap walk
   int last_handle_cells = 0;        // ... and cells served by their own filtered launch instead of the fused walk
   std::vector<int64_t> below;       // annb_cellset_set_bruteforce: per cell, scan filters admitting <= this many (-1 = never)
-  int64_t last_scanned_pairs = 0;   // (query, cell) pairs the last filtered search scanned exactly ...
+  int64_t last_scanned_pairs = 0;   // (query, cell) pairs the last search scanned exactly ...
   int64_t last_scanned_rows = 0;    // ... and the rows those scans scored
   CellBuildStats build;             // annb_cellset_add_items: the last call's one-pass build ...
   int build_cells = 0;              // ... and the cells it served
@@ -39,8 +39,8 @@ namespace {
 
 enum { C_QUERIES = 0, C_ORDER, C_K, C_LABELS, C_DISTS, C_FOUND, C_STATS, C_OUT, C_BITS, C_TABLES, C_TMP_L, C_TMP_D, C_TMP_F,
        C_TMP_S, C_QMAP, C_SLOT, C_SLOT_K, C_SLOT_BITS, C_GTABLES, C_QF, C_SCAN_JOBS, C_SCAN_ROWS, C_SCAN_QUERIES,
-       C_SCAN_BLOCKS };
-static_assert(C_SCAN_BLOCKS < 24, "annb_cellset::buf is too small");
+       C_SCAN_BLOCKS, C_SCAN_PARTS, C_SCAN_DONE };
+static_assert(C_SCAN_DONE < 26, "annb_cellset::buf is too small");
 
 int cs_buf(annb_cellset *cs, int slot, size_t bytes, void **out) {
   if (bytes == 0) bytes = 16;
@@ -416,15 +416,18 @@ int merge_and_finish(annb_cellset *cs, const float *sd, const uint64_t *sl, cons
   return ANNB_OK;
 }
 
-// One exact subset scan of a filtered cell-set search: cell `cell`'s prepared filter `f` (its admitted rows in id
-// order, or a label list's live entries in order) scanned for the query rows `rows` with k results each.
+// One exact subset scan of a cell-set search: cell `cell`'s prepared filter `f` (its admitted rows in id order, or a
+// label list's live entries in order), or with f == nullptr the cell's `live` rows in id order (`dead` = its deletion
+// bitmap, nullptr when nothing is deleted), scanned for the query rows `rows` with k results each.
 struct ScanPlan {
   int cell = 0, k = 0;
   const PreparedFilter *f = nullptr;
+  int64_t live = 0;
+  const uint32_t *dead = nullptr;
   std::vector<uint32_t> rows;
 };
 
-int64_t plan_rows(const ScanPlan &p) { return p.f->ids ? p.f->n_ids : p.f->count; }
+int64_t plan_rows(const ScanPlan &p) { return !p.f ? p.live : (p.f->ids ? p.f->n_ids : p.f->count); }
 
 // a scanned pair with fewer live subset entries than its k fails as annb_scan_subset fails
 int check_plans(const std::vector<ScanPlan> &plans) {
@@ -439,8 +442,10 @@ struct StagedScans {
   std::vector<SubsetScan> jobs;
   std::vector<std::pair<size_t, size_t>> groups;  // [first, last) jobs of each launch
   std::vector<int64_t> tile0;                     // first tile of each launch (+ the end)
+  std::vector<SubsetChunks> chunks;               // each launch's row chunks
+  std::vector<int64_t> tile_groups;               // ... and its (job, first query) tiles, whose counters it zeroes
   SubsetScan *djobs = nullptr;
-  int2 *dtiles = nullptr;
+  int4 *dtiles = nullptr;
 };
 
 // The plans (in cell order) staged on the cell set's stream, before the walk: one gather and one scan for all plans, or
@@ -452,8 +457,9 @@ int stage_scans(annb_cellset *cs, const std::vector<ScanPlan> &plans, const std:
   cudaStream_t st = cs->h0->stream;
   int64_t rows = 0, blocks = 0, nq = 0;
   for (const ScanPlan &p : plans) {
-    rows += plan_rows(p);
-    if (!p.f->ids) blocks += ((p.f->n + 31) / 32 + 255) / 256;
+    const int64_t span = p.f ? p.f->n : gd[(size_t)p.cell].n;  // ids a bitmap covers
+    if (p.f || p.dead) rows += plan_rows(p);                   // (a live-rows plan without deletions is scanned in place)
+    if (p.f ? !p.f->ids : p.dead != nullptr) blocks += ((span + 31) / 32 + 255) / 256;
     nq += (int64_t)p.rows.size();
   }
   // launch groups: [g0, g1) ranges of plans, each with its tiles
@@ -461,27 +467,62 @@ int stage_scans(annb_cellset *cs, const std::vector<ScanPlan> &plans, const std:
   for (size_t j = 0; j < J; j++)
     if (groups.empty() || (per_cell && plans[j].cell != plans[groups.back().first].cell)) groups.push_back({j, j + 1});
     else groups.back().second = j + 1;
-  std::vector<int2> tiles;
+  // tiles {job in the launch, first query, chunk, tile group}: a launch whose tiles are too few to fill the GPU cuts its
+  // subsets into row chunks (subset_scan_chunk_rows); its chunk lists take (tile groups, width, G, K) entries
+  std::vector<int4> tiles;
   std::vector<int64_t> &tile0 = ss.tile0;
+  size_t part_entries = 0, max_groups = 0;
   for (auto &g : groups) {
     int kmax = 1;
     for (size_t j = g.first; j < g.second; j++) kmax = std::max(kmax, plans[j].k);
     const int w = subset_scan_tile_width(kmax);
+    int64_t n_groups = 0, longest = 0;
+    for (size_t j = g.first; j < g.second; j++) {
+      n_groups += ((int64_t)plans[j].rows.size() + w - 1) / w;
+      if (!plans[j].rows.empty()) longest = std::max(longest, plan_rows(plans[j]));
+    }
+    SubsetChunks ch;
+    memset(&ch, 0, sizeof(ch));
+    ch.rows = subset_scan_chunk_rows(cs->h0, n_groups, longest);
+    ch.K = kmax;
+    ch.G = ch.rows ? (int)((longest + ch.rows - 1) / ch.rows) : 1;
     tile0.push_back((int64_t)tiles.size());
-    for (size_t j = g.first; j < g.second; j++)
-      for (size_t q0 = 0; q0 < plans[j].rows.size(); q0 += (size_t)w) tiles.push_back(make_int2((int)(j - g.first), (int)q0));
+    int group = 0;
+    for (size_t j = g.first; j < g.second; j++) {
+      const int nch = ch.rows ? (int)((plan_rows(plans[j]) + ch.rows - 1) / ch.rows) : 1;
+      for (size_t q0 = 0; q0 < plans[j].rows.size(); q0 += (size_t)w, group++)
+        for (int c = 0; c < nch; c++) tiles.push_back(make_int4((int)(j - g.first), (int)q0, c, group));
+    }
+    if (ch.rows) {
+      part_entries = std::max(part_entries, (size_t)n_groups * w * ch.G * ch.K);
+      max_groups = std::max(max_groups, (size_t)n_groups);
+    }
+    ss.chunks.push_back(ch);
+    ss.tile_groups.push_back(n_groups);
   }
   tile0.push_back((int64_t)tiles.size());
+  if (part_entries) {
+    void *pp;
+    unsigned int *done;
+    ANNB_TRY_RC(cs_buf(cs, C_SCAN_PARTS, part_entries * 8, &pp));
+    ANNB_TRY_RC(cs_buf(cs, C_SCAN_DONE, max_groups * 4, (void **)&done));
+    for (SubsetChunks &ch : ss.chunks)
+      if (ch.rows) {
+        ch.part_d = (float *)pp;
+        ch.part_i = reinterpret_cast<uint32_t *>((float *)pp + part_entries);
+        ch.done = done;
+      }
+  }
   uint64_t *glab;
   uint32_t *dq;
   unsigned int *boffs;
   SubsetScan *djobs;
-  const size_t qwords = ((size_t)nq + 1) / 2 * 2;
+  const size_t qwords = ((size_t)nq + 3) / 4 * 4;  // the int4 tiles follow the query rows: 16-byte aligned
   ANNB_TRY_RC(cs_buf(cs, C_SCAN_ROWS, (size_t)rows * 16, (void **)&glab));
-  ANNB_TRY_RC(cs_buf(cs, C_SCAN_QUERIES, qwords * 4 + tiles.size() * sizeof(int2), (void **)&dq));
+  ANNB_TRY_RC(cs_buf(cs, C_SCAN_QUERIES, qwords * 4 + tiles.size() * sizeof(int4), (void **)&dq));
   ANNB_TRY_RC(cs_buf(cs, C_SCAN_BLOCKS, (size_t)blocks * 4, (void **)&boffs));
   ANNB_TRY_RC(cs_buf(cs, C_SCAN_JOBS, J * sizeof(SubsetScan), (void **)&djobs));
-  int2 *dtiles = reinterpret_cast<int2 *>(dq + qwords);
+  int4 *dtiles = reinterpret_cast<int4 *>(dq + qwords);
   uint8_t *gcodes = reinterpret_cast<uint8_t *>(glab + rows);
   std::vector<SubsetScan> &jobs = ss.jobs;
   jobs.resize(J);
@@ -492,20 +533,32 @@ int stage_scans(annb_cellset *cs, const std::vector<ScanPlan> &plans, const std:
     const ScanPlan &p = plans[j];
     SubsetScan &s = jobs[j];
     memset(&s, 0, sizeof(s));
-    s.bits = p.f->ids ? nullptr : p.f->bits;
-    s.ids = p.f->ids;
-    s.nwords = (p.f->n + 31) / 32;
     s.cell_codes = own[p.cell];
     s.cell_labels = gd[p.cell].labels;
     s.codes = gcodes + r0 * 8;
     s.labels = glab + r0;
+    if (p.f) {
+      s.kind = SUBSET_FILTER;
+      s.bits = p.f->ids ? nullptr : p.f->bits;
+      s.ids = p.f->ids;
+      s.nwords = (p.f->n + 31) / 32;
+    } else {
+      s.kind = SUBSET_LIVE;
+      s.bits = p.dead;
+      s.n_rows = gd[p.cell].n;
+      s.nwords = (s.n_rows + 31) / 32;
+      if (!p.dead) {  // every row, read where it is (the kernels only read a subset's codes and labels)
+        s.codes = const_cast<uint8_t *>(s.cell_codes);
+        s.labels = const_cast<uint64_t *>(s.cell_labels);
+      }
+    }
     s.block_offs = boffs + bl0;
     s.n = plan_rows(p);
     s.queries = dq + hq.size();
     s.nq = (int32_t)p.rows.size();
     s.k = p.k;
     s.cell = p.cell;
-    r0 += s.n;
+    if (s.bits || s.ids) r0 += s.n;
     if (s.bits) bl0 += (s.nwords + 255) / 256;
     hq.insert(hq.end(), p.rows.begin(), p.rows.end());
     cs->last_scanned_pairs += s.nq;
@@ -513,7 +566,7 @@ int stage_scans(annb_cellset *cs, const std::vector<ScanPlan> &plans, const std:
   }
   ANNB_CUDA(cudaMemcpyAsync(djobs, jobs.data(), J * sizeof(SubsetScan), cudaMemcpyHostToDevice, st));
   ANNB_CUDA(cudaMemcpyAsync(dq, hq.data(), hq.size() * 4, cudaMemcpyHostToDevice, st));
-  ANNB_CUDA(cudaMemcpyAsync(dtiles, tiles.data(), tiles.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+  ANNB_CUDA(cudaMemcpyAsync(dtiles, tiles.data(), tiles.size() * sizeof(int4), cudaMemcpyHostToDevice, st));
   ss.djobs = djobs;
   ss.dtiles = dtiles;
   return ANNB_OK;  // (pageable sources: each copy has taken its data when it returns)
@@ -524,22 +577,30 @@ int launch_scans(annb_cellset *cs, const StagedScans &ss, const float *tables, c
   for (size_t g = 0; g < ss.groups.size(); g++) {
     const size_t j0 = ss.groups[g].first, j1 = ss.groups[g].second;
     const std::vector<SubsetScan> part(ss.jobs.begin() + (ptrdiff_t)j0, ss.jobs.begin() + (ptrdiff_t)j1);
+    const SubsetChunks &ch = ss.chunks[g];
+    if (ch.rows) ANNB_CUDA(cudaMemsetAsync(ch.done, 0, (size_t)ss.tile_groups[g] * 4, cs->h0->stream));
     ANNB_TRY_RC(launch_subset_scan(cs->h0, cs->h0->stream, ss.djobs + j0, part, ss.dtiles + ss.tile0[g], ss.tile0[g + 1] - ss.tile0[g],
-                                   tables, cs->n_cells, limit, b.sl, b.sd, b.sfound, b.sstats));
+                                   ch, tables, cs->n_cells, limit, b.sl, b.sd, b.sfound, b.sstats));
   }
   return ANNB_OK;
 }
 
-// cell c's filter `f` is scanned rather than walked: its threshold is set and the filter admits at most that many
-// (`need_rows`: and at least one); the scan's geometry and the cell's own codes are checked / made current here
-int scan_decision(annb_cellset *cs, int c, const PreparedFilter *f, bool need_rows, std::vector<const uint8_t *> &own, bool *out) {
-  const int64_t lim = cs->below.empty() ? -1 : cs->below[(size_t)c];
-  *out = lim >= 0 && f->count <= lim && (!need_rows || f->count > 0);
-  if (!*out || own[(size_t)c]) return ANNB_OK;
+// cell c is scanned: the scan's geometry and the cell's own codes are checked / made current here
+int scan_cell(annb_cellset *cs, int c, std::vector<const uint8_t *> &own) {
+  if (own[(size_t)c]) return ANNB_OK;
   annb_index *h = cs->cells[(size_t)c];
   if (!subset_scan_applicable(h))
     ANNB_FAIL(ANNB_ELIMIT, "cell %d: the exact subset scan needs M = 8 one-byte codes with 256 centroids", c);
   return sync_own_codes(h, &own[(size_t)c]);
+}
+
+// cell c's filter `f` is scanned rather than walked: its threshold is set (ANNB_CELLS_EXACT: +inf) and the filter
+// admits at most that many (`need_rows`: and at least one)
+int scan_decision(annb_cellset *cs, int c, const PreparedFilter *f, bool need_rows, bool exact, std::vector<const uint8_t *> &own,
+                  bool *out) {
+  const int64_t lim = exact ? INT64_MAX : (cs->below.empty() ? -1 : cs->below[(size_t)c]);
+  *out = lim >= 0 && f->count <= lim && (!need_rows || f->count > 0);
+  return *out ? scan_cell(cs, c, own) : ANNB_OK;
 }
 
 // The argument checks of a cell-set search: `bad` = the entry point's own check of B, limit, ef and its pointers,
@@ -585,6 +646,21 @@ int batch_tables(annb_cellset *cs, Staged &b, int64_t B) {
   ANNB_TRY_RC(cs_buf(cs, C_TABLES, (size_t)B * h0->M * h0->Ks * sizeof(float), (void **)&b.tables));
   std::lock_guard<std::mutex> lk(h0->mu);
   return launch_adc_table(h0, b.dq, B, b.tables);
+}
+
+// ANNB_CELLS_EXACT: the plans scanned and nothing walked, one launch for all of them (per_cell: one per cell), timed
+// as the walk
+int run_exact(annb_cellset *cs, Staged &b, int64_t B, int normalize, int limit, const std::vector<ScanPlan> &plans,
+              const std::vector<const uint8_t *> &own, const std::vector<GraphDev> &gd, bool per_cell) {
+  cudaStream_t st = cs->h0->stream;
+  for (int r = 0; r < normalize; r++) ANNB_TRY_RC(launch_l2_normalize(cs->h0, b.dq, B, cs->dim));
+  StagedScans ss;
+  ANNB_TRY_RC(stage_scans(cs, plans, own, gd, per_cell, ss));
+  if (!plans.empty()) ANNB_TRY_RC(batch_tables(cs, b, B));
+  cudaEventRecord(cs->ev[2], st);
+  if (!plans.empty()) ANNB_TRY_RC(launch_scans(cs, ss, b.tables, b, limit));
+  cudaEventRecord(cs->ev[3], st);
+  return ANNB_OK;
 }
 
 // One launch of cell c on its own handle's stream (after everything queued on the cell set's, which waits for it in
@@ -750,20 +826,51 @@ int annb_cellset_search(annb_cellset_t *cs, const float *queries, int in_space, 
                            "bad B / limit / ef / outputs", false, B, order, in_space, n_probe, limit, ef));
   const int C = cs->n_cells;
   annb_index *h0 = cs->h0;
+  const bool exact = flags & ANNB_CELLS_EXACT;
   std::vector<GraphDev> gd;
   std::vector<int32_t> kc(C);
+  std::vector<int64_t> live(C);
+  std::vector<const uint32_t *> dead(C, nullptr);
+  std::vector<const uint8_t *> own_codes(C, nullptr);
   bool fused = !(flags & ANNB_CELLS_GENERIC);
   ANNB_TRY_RC(sync_cells(cs, gd, [&](int c, annb_index *h) {
-    const int64_t live = h->g.count.load() - h->g.num_deleted;
-    kc[c] = (int32_t)std::min<int64_t>(limit, std::max<int64_t>(live, 0));  // container.py:104-105, :119
+    live[c] = std::max<int64_t>(h->g.count.load() - h->g.num_deleted, 0);
+    kc[c] = (int32_t)std::min<int64_t>(limit, live[c]);  // container.py:104-105, :119
+    if (exact) {
+      if (h->g.num_deleted > 0) dead[c] = gd[c].deleted;
+      return kc[c] > 0 || !subset_scan_applicable(h) ? scan_cell(cs, c, own_codes) : ANNB_OK;
+    }
     fused &= h->g.num_deleted == 0 && !h->opt_force_general && walk4_can_fuse(h) && h->M == 8;
     return ANNB_OK;
   }));
   cs->last_route = fused ? 0 : 1;
+  cs->last_scanned_pairs = 0;
+  cs->last_scanned_rows = 0;
   if (B == 0) return ANNB_OK;
   cudaStream_t st = h0->stream;
   Staged b;
   ANNB_TRY_RC(stage_batch(cs, queries, in_space, B, order, n_probe, limit, part_stats != nullptr, b));
+  if (exact) {
+    // every probed cell with k > 0 scanned over its live rows for the queries that probe it
+    std::vector<int32_t> otmp;
+    const int32_t *ho;
+    ANNB_TRY_RC(host_order(cs, order, in_space, b.dorder, B, n_probe, otmp, &ho));
+    std::vector<ScanPlan> plans(C);
+    for (int c = 0; c < C; c++) {
+      plans[c].cell = c;
+      plans[c].k = kc[c];
+      plans[c].live = live[c];
+      plans[c].dead = dead[c];
+    }
+    for (int64_t q = 0; q < B; q++)
+      for (int i = 0; i < n_probe; i++) plans[(size_t)ho[q * n_probe + i]].rows.push_back((uint32_t)q);
+    std::vector<ScanPlan> kept;
+    for (ScanPlan &p : plans)
+      if (p.k > 0 && !p.rows.empty()) kept.push_back(std::move(p));
+    ANNB_TRY_RC(run_exact(cs, b, B, normalize, limit, kept, own_codes, gd, !fused));
+    return merge_and_finish(cs, b.sd, b.sl, b.sfound, b.sstats, b.dorder, !order, B, n_probe, limit, labels_out, dists_out, cells_out,
+                            out_space, part_labels, part_dists, part_stats);
+  }
   float *dq = b.dq;
   int32_t *dorder = b.dorder, *sfound = b.sfound;
   uint64_t *sl = b.sl;
@@ -822,8 +929,10 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
   std::vector<const PreparedFilter *> pfs(C, nullptr);
   std::vector<char> scan(C, 0);  // 1 = the cell's subset is scanned exactly (annb_cellset_set_bruteforce)
   std::vector<const uint8_t *> own_codes(C, nullptr);
+  const bool exact = flags & ANNB_CELLS_EXACT;
   bool fused = !(flags & ANNB_CELLS_GENERIC);
   ANNB_TRY_RC(sync_cells(cs, gd, [&](int c, annb_index *h) {
+    if (exact && !subset_scan_applicable(h)) return scan_cell(cs, c, own_codes);  // (fails: the scan's geometry)
     if (filter_ids[c] != 0) {
       PreparedFilter *f;
       const int rc = find_prepared_filter(h, filter_ids[c], &f);
@@ -838,11 +947,11 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       sel[c] = (float)std::min<double>(1.0, (double)f->count / (double)std::max<int64_t>(1, h->gd.n));
       pfs[c] = f;
       bool sc;
-      ANNB_TRY_RC(scan_decision(cs, c, f, true, own_codes, &sc));
+      ANNB_TRY_RC(scan_decision(cs, c, f, true, exact, own_codes, &sc));
       scan[c] = sc;
     }
     int ep, en;
-    fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
+    if (!exact) fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
     return ANNB_OK;
   }));
   // fused route: the cells hnsw_walk4f serves, and N's size (the largest any of them needs alone)
@@ -895,7 +1004,9 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       }
     ANNB_TRY_RC(check_plans(plans));
   }
-  if (!fused) {
+  if (exact) {
+    ANNB_TRY_RC(run_exact(cs, b, B, normalize, limit, plans, own_codes, gd, !fused));
+  } else if (!fused) {
     // one annb_search_prepared per probed cell that is not scanned; a walk with fewer than k_c results fails the call as
     // it fails the cell
     std::vector<int32_t> kpc(kc);
@@ -1014,10 +1125,14 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
   std::vector<const PreparedFilter *> spf((size_t)(S * C), nullptr);
   std::vector<char> sscan((size_t)(S * C), 0);  // 1 = the pair's subset is scanned exactly (annb_cellset_set_bruteforce)
   std::vector<const uint8_t *> own_codes(C, nullptr);
+  std::vector<int64_t> nlive(C);
+  const bool exact = flags & ANNB_CELLS_EXACT;
   bool fused = !(flags & ANNB_CELLS_GENERIC);
   ANNB_TRY_RC(sync_cells(cs, gd, [&](int c, annb_index *h) {
+    if (exact && !subset_scan_applicable(h)) return scan_cell(cs, c, own_codes);  // (fails: the scan's geometry)
     ndel[c] = h->g.num_deleted;
     const int64_t live = std::max<int64_t>(h->g.count.load() - h->g.num_deleted, 0);
+    nlive[c] = live;
     const double nn = (double)std::max<int64_t>(1, h->gd.n);
     std::unordered_map<int, const PreparedFilter *> pf;
     for (int64_t s = 0; s < S; s++) {
@@ -1026,6 +1141,10 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       if (id == 0) {  // annb_search_multi's unfiltered rows: the live rows (k = min(limit, live), container.py:119)
         sk[i] = (int32_t)std::min<int64_t>(limit, live);
         ssel[i] = (float)(1.0 - (double)h->g.num_deleted / nn);
+        if (exact && sk[i] > 0) {  // ANNB_CELLS_EXACT: scanned over the cell's live rows
+          sscan[i] = 1;
+          ANNB_TRY_RC(scan_cell(cs, c, own_codes));
+        }
         continue;
       }
       auto it = pf.find(id);
@@ -1046,11 +1165,11 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       ssel[i] = (float)std::min<double>(1.0, (double)f->count / nn);
       spf[i] = f;
       bool sc;
-      ANNB_TRY_RC(scan_decision(cs, c, f, false, own_codes, &sc));
+      ANNB_TRY_RC(scan_decision(cs, c, f, false, exact, own_codes, &sc));
       sscan[i] = sc;
     }
     int ep, en;
-    fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
+    if (!exact) fused &= walk4_can_fuse(h) && h->M == 8 && h->opt_force_general != 2 && walk4f_geometry(h, ef_max, 1.0, &ep, &en);
     return ANNB_OK;
   }));
   cs->last_route = fused ? 0 : 1;
@@ -1062,7 +1181,8 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
   cudaStream_t st = h0->stream;
   Staged b;
   ANNB_TRY_RC(stage_batch(cs, queries, in_space, B, order, n_probe, limit, part_stats != nullptr, b));
-  for (int r = 0; r < normalize; r++) ANNB_TRY_RC(launch_l2_normalize(h0, b.dq, B, cs->dim));
+  if (!exact)
+    for (int r = 0; r < normalize; r++) ANNB_TRY_RC(launch_l2_normalize(h0, b.dq, B, cs->dim));
   std::vector<int32_t> otmp;
   const int32_t *ho;
   ANNB_TRY_RC(host_order(cs, order, in_space, b.dorder, B, n_probe, otmp, &ho));
@@ -1080,13 +1200,20 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
         ScanPlan &pl = by_filter[{c, row_id(slot[(size_t)q], c)}];
         pl.cell = c;
         pl.k = sk[sc];
-        pl.f = spf[sc];
+        pl.f = spf[sc];  // (nullptr: no filter, the live rows)
+        pl.live = nlive[c];
+        pl.dead = ndel[c] > 0 ? gd[c].deleted : nullptr;
         pl.rows.push_back((uint32_t)q);
       }
     }
   std::vector<ScanPlan> plans;
   for (auto &kv : by_filter) plans.push_back(std::move(kv.second));
   ANNB_TRY_RC(check_plans(plans));
+  if (exact) {
+    ANNB_TRY_RC(run_exact(cs, b, B, normalize, limit, plans, own_codes, gd, !fused));
+    return merge_and_finish(cs, b.sd, b.sl, b.sfound, b.sstats, b.dorder, !order, B, n_probe, limit, labels_out, dists_out, cells_out,
+                            out_space, part_labels, part_dists, part_stats);
+  }
   // fused route: the pairs hnsw_walk4f serves, and N's size (the largest any of them needs alone)
   std::vector<char> own((size_t)(S * C), 0);  // 1 = the pair goes to its cell's own launch
   int ep = ef_max <= 64 ? 2 : 4, en = 0;

@@ -538,7 +538,7 @@ class CellSet:
             pass
 
     def search(self, queries, limit=10, ef=50, normalize=0, order=None, n_probe=None, generic=False, with_parts=False,
-               filter_ids=None, query_filter_ids=None, bruteforce_below=None):
+               filter_ids=None, query_filter_ids=None, bruteforce_below=None, exact=False):
         """-> (labels uint64 (B, limit), dists fp32 (B, limit), cells int32 (B, limit)) [+ (part labels, part dists,
         part counters) (B, n_cells, limit / 3)].  `order` = (B, n_probe) cells per query, or None for the centroids'.
         `filter_ids` = one prepared filter id per cell (of that cell's Engine; 0 = the cell admits nothing), or None
@@ -547,7 +547,9 @@ class CellSet:
         (annb_cellset_search_multi); exclusive with `filter_ids`.  `bruteforce_below` = (n_cells,) thresholds for the
         filtered forms (HnswIndex.bruteforce_filter_below per cell, -1 = none), None = none: a cell's filter (or a
         query's filter in a cell) that admits at most that many rows is scanned exactly instead of walked
-        (annb_cellset_set_bruteforce)."""
+        (annb_cellset_set_bruteforce).  `exact` = IVF-PQ with exact ADC top-k inside the probed cells
+        (ANNB_CELLS_EXACT): every probed (query, cell) pair is scanned exactly over the rows it admits (the cell's live
+        rows, or the filter's subset) and nothing is walked; `ef` is then unused."""
         below = None
         if bruteforce_below is not None:
             below = np.ascontiguousarray(bruteforce_below, dtype=np.int64).reshape(-1)
@@ -574,7 +576,7 @@ class CellSet:
         if order is not None and qs == L.DEVICE:
             raise ValueError('pass the probe order with host queries')
         head = (self._h, qp, qs, B, int(normalize), order.ctypes.data if order is not None else None, n_probe, int(limit),
-                int(ef), L.CELLS_GENERIC if generic else 0)
+                int(ef), (L.CELLS_GENERIC if generic else 0) | (L.CELLS_EXACT if exact else 0))
         tail = (labels.ctypes.data, dists.ctypes.data, cells.ctypes.data, L.HOST,
                 *([p.ctypes.data for p in parts] if parts else [None, None, None]))
         if filter_ids is not None and query_filter_ids is not None:

@@ -407,6 +407,16 @@ ANNB_API int annb_lane_stream(annb_index_t *h, int lane, uint64_t *stream_out);
  * concatenation position), a stable form of container.py:135. */
 #define ANNB_MAX_CELLS 256
 #define ANNB_CELLS_GENERIC 1 /* annb_cellset_search flag: take the per-cell route even where the fused walk applies */
+/* annb_cellset_search* flag: IVF-PQ with exact ADC top-k inside the probed cells.  Every probed (query, cell) pair with
+ * k > 0 is scanned exactly over the rows it admits, and nothing is walked (ef is unused): without a filter (and in
+ * annb_cellset_search_multi for filter id 0) the cell's live rows in internal-id order; with a filter, its subset as
+ * annb_cellset_set_bruteforce defines it (a label list keeps its order and repeats).  k is the walk's, min(limit, live
+ * rows, admitted count).  Each pair's part is annb_scan_subset over that subset -- ids, distance bits and order, with
+ * counters {0, 0, rows scored} -- and the merge is the walk's.  In the filtered forms the flag acts as thresholds of
+ * +inf for this call only (the stored ones are kept).  One scan launch serves every pair (route 0), or one per cell
+ * with ANNB_CELLS_GENERIC (route 1); a small batch over large subsets has its subsets split into row chunks, merged in
+ * the same launch, with the same results.  The scan needs M = 8 one-byte codes with Ks = 256 (else ANNB_ELIMIT). */
+#define ANNB_CELLS_EXACT 2
 typedef struct annb_cellset annb_cellset_t;
 ANNB_API int annb_cellset_create(annb_index_t *const *handles, int n_cells, const float *centroids, int metric,
                         annb_cellset_t **out);
@@ -462,8 +472,8 @@ ANNB_API int annb_cellset_last_filtered(annb_cellset_t *cs, int64_t *rerun_pairs
  * needs M = 8 one-byte codes with Ks = 256 (else ANNB_ELIMIT).  A scanned pair's part counters are {0 hops,
  * 0 neighbours listed, rows scored}. */
 ANNB_API int annb_cellset_set_bruteforce(annb_cellset_t *cs, const int64_t *below);
-/* The (query, cell) pairs the last annb_cellset_search_prepared / annb_cellset_search_multi scanned exactly, and the
- * rows those scans scored (the sum over scanned pairs of their subset's size). */
+/* The (query, cell) pairs the last annb_cellset_search* call scanned exactly (bruteforce thresholds, ANNB_CELLS_EXACT),
+ * and the rows those scans scored (the sum over scanned pairs of their subset's size). */
 ANNB_API int annb_cellset_last_scanned(annb_cellset_t *cs, int64_t *pairs, int64_t *rows);
 ANNB_API int annb_cellset_merge(annb_cellset_t *cs, const uint64_t *labels, const float *dists, const int32_t *counts,
                        const int32_t *order, int in_space, int64_t B, int n_probe, int limit, uint64_t *labels_out,
@@ -471,8 +481,9 @@ ANNB_API int annb_cellset_merge(annb_cellset_t *cs, const uint64_t *labels, cons
 /* The probe order alone: (B, n_probe) int32 cells per query, nearest centroid first. */
 ANNB_API int annb_cellset_probe(annb_cellset_t *cs, const float *queries, int in_space, int64_t B, int n_probe,
                        int32_t *order_out, int out_space);
-/* Device time of the last probe / walk (fused launch, or the per-cell searches) / merge in ms, and the route the last
- * annb_cellset_search* call took (0 = fused walk, 1 = per-cell searches; annb_cellset_search_multi: own launches). */
+/* Device time of the last probe / walk (fused launch, or the per-cell searches; ANNB_CELLS_EXACT: the scans) / merge in
+ * ms, and the route the last annb_cellset_search* call took (0 = fused walk or one scan launch, 1 = per-cell searches or
+ * one scan launch per cell; annb_cellset_search_multi: own launches). */
 ANNB_API int annb_cellset_last_ms(annb_cellset_t *cs, float *probe_ms, float *walk_ms, float *merge_ms, int *route);
 /* Insertion into a cell set: host fp32 rows (n, dim), their labels and a target cell per row (int32).  Rows are split
  * by cell, each cell keeping its rows in input order, and every cell's graph comes out exactly as
@@ -537,7 +548,9 @@ ANNB_API int annb_device_graph_export(annb_index_t *h, int part, void *dst, int6
  * traversed-only list to 32 x value entries), "flagged_epl" (force hnsw_walk_flagged with 32 x value entries),
  * "force_general" (1 = filtered route without a filter, 2 = bitmap walk), "scan_kernel" (K2: 0 query-tiled where it
  * applies, 1 round-1 kernel, 2 tiled even for small inputs, 3 first tiled version), "warps_per_cta", "ctas_per_sm",
- * "gpu_build", "gpu_build_frac", "timing", "ip_raw", "dump_tables", "reset_counters". */
+ * "gpu_build", "gpu_build_frac", "timing", "ip_raw", "dump_tables", "reset_counters", "subset_chunk_rows" (on a cell
+ * set's first handle: its exact subset scans in row chunks of value rows, raised so no subset has more than 16; -1 =
+ * never chunked; 0 = by size, the default). */
 ANNB_API int annb_set_option(annb_index_t *h, const char *name, int64_t value);
 
 #ifdef __cplusplus
