@@ -395,6 +395,13 @@ int launch_scatter_records(annb_index *h, const uint8_t *d_staged, const uint32_
 // mode: 0 = fast walk (no filter, no deletions), 1 = filtered/deleted walk, kernel chosen automatically
 // (flagged single-list walk when its list fits, else the bitmap walk), 2 = bitmap walk
 int launch_search(annb_index *h, const SearchParams &p, int mode);
+// The route launch_search takes for rows with a filter (filtered) or without, at ef, whose lists are sized by
+// `selectivity` (search_selectivity): returns the mode -- 0 = no filter and no deletions, 1, or 2 under
+// opt_force_general == 2 -- with *fuse = the walk builds its own tables from the queries (no K1 launch, no (B, M, Ks)
+// buffer) and *walk4f = the rows take mode 1 on hnsw_walk4f (either pointer may be null)
+int search_route(const annb_index *h, int ef, bool filtered, double selectivity, bool *fuse, bool *walk4f);
+// the fraction of the nodes a search can admit: a filter's `count` rows, or (not filtered) the rows not deleted
+double search_selectivity(const annb_index *h, bool filtered, int64_t count);
 // the work counter of a walk launch and the overflow flag behind it (p.work_counter, or scratch slot 4 when the caller
 // passes none; a caller running several launches concurrently passes its own), zeroed on h->stream
 int walk_counter(annb_index *h, SearchParams &p);
@@ -424,6 +431,8 @@ int launch_walk4_cells(annb_index *h, const SearchParams &p);
 bool walk4f_applicable(const annb_index *h, int ef, double selectivity);
 // ... and its list geometry for that search: (ep, en) = entries per lane of P and N; false = not applicable
 bool walk4f_geometry(const annb_index *h, int ef, double selectivity, int *ep_out, int *en_out);
+// N's entries per lane as instantiated beside P's ep: the smallest geometry with at least en (en > 0)
+int walk4f_round_en(int ep, int en);
 int launch_walk4f(annb_index *h, const SearchParams &p);
 // the filtered multi-cell walk with lists of (ep, en) entries per lane; returns 1 = not instantiated for these
 int launch_walk4f_cells(annb_index *h, const SearchParams &p, int ep, int en);

@@ -310,17 +310,6 @@ static int64_t table_chunk_rows(const annb_index *h, int64_t B) {
   return std::max<int64_t>(1, std::min<int64_t>(B, (int64_t)(cap / per)));
 }
 
-// fill the fused-build fields of a SearchParams (hnsw_walk4 builds each query's table in shared memory)
-static void fuse_params(annb_index *h, SearchParams &p, const float *d_queries) {
-  p.tables = nullptr;
-  p.queries = d_queries;
-  p.cbt = h->d_codebook_t;
-  p.cb_vec = h->cb_vec;
-  p.ds = h->ds;
-  p.is_ip = h->metric != ANNB_METRIC_L2;
-  p.bias = h->opt_ip_raw ? 0.f : (float)(1.0 / (double)h->Ks);
-}
-
 int annb_adc_table(annb_index_t *h, const float *queries, int q_space, int64_t B, int normalize, float *out, int out_space) {
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
@@ -1198,6 +1187,51 @@ static int batch_outputs(annb_index *h, const MultiBatch &mb) {
   return ANNB_OK;
 }
 
+// A batch's rows in launches: one group for a batch under one filter (or none), three for a batch with one filter per
+// query (annb_search_multi): 0 = no filter (the plain walk, or the deletion-aware one), 1 = filters hnsw_walk4f takes
+// (its list N sized by the group's smallest selectivity, so one selective filter does not move every query to the
+// round-1 kernel), 2 = the other filtered rows (hnsw_walk_flagged / the bitmap walk).  Each group is ONE launch over its
+// rows, contiguous in the batch's (gathered) row order.
+struct MultiGroup {
+  int64_t o = 0, n = 0;  // gathered rows [o, o + n)
+  bool filtered = false;
+  double s = 1.0;        // the selectivity the group's lists are sized by
+  int mode = 0;          // launch_search mode
+  bool fuse = false;     // tables built inside the walk (else read from `tables`)
+};
+
+// The walk launch of group g of batch mb over the batch's (B, M, Ks) `tables` or, fused, its queries; `dump`: the
+// tables it used go to opt_dump_tables, at the group's rows
+static SearchParams walk_params(const annb_index *h, const MultiBatch &mb, const MultiGroup &g, const float *tables, bool dump,
+                                unsigned int *work_counter) {
+  const size_t TS = (size_t)h->M * h->Ks;
+  SearchParams p;
+  memset(&p, 0, sizeof(p));
+  if (g.fuse) {  // hnsw_walk4 / hnsw_walk4f build each query's table in shared memory
+    p.queries = mb.dq + g.o * h->dim;
+    p.cbt = h->d_codebook_t;
+    p.cb_vec = h->cb_vec;
+    p.ds = h->ds;
+    p.is_ip = h->metric != ANNB_METRIC_L2;
+    p.bias = h->opt_ip_raw ? 0.f : (float)(1.0 / (double)h->Ks);
+  } else {
+    p.tables = tables + g.o * TS;
+  }
+  if (dump && h->opt_dump_tables) p.dump_tables = reinterpret_cast<float *>(h->opt_dump_tables) + g.o * TS;
+  p.B = g.n;
+  p.k = mb.k;
+  p.ef = mb.ef;
+  p.filter = mb.filter;
+  p.query_filter = g.filtered && mb.dqf ? mb.dqf + g.o : nullptr;
+  p.selectivity = (float)g.s;
+  p.out_labels = mb.gl + g.o * mb.k;
+  p.out_dists = mb.gd + g.o * mb.k;
+  p.out_found = mb.gfound + g.o;
+  p.out_stats = mb.gstats ? mb.gstats + g.o * 3 : nullptr;
+  p.work_counter = work_counter;
+  return p;
+}
+
 // The queries of a settled batch that outgrew the flagged walk's list (found = -1, n_over of them) re-run on the bitmap
 // walk (exact, any size) through a query-row map, with their own bitmaps, on h->stream: only their rows of the outputs
 // are overwritten, then the outputs are copied back again.
@@ -1216,19 +1250,11 @@ static int rerun_flagged(annb_index *h, MultiBatch &mb, int64_t n_over) {
     ANNB_TRY(launch_adc_table(h, mb.dq, mb.B, t));
     tables = t;
   }
-  SearchParams p;
-  memset(&p, 0, sizeof(p));
-  p.tables = tables;
-  p.B = n_over;
-  p.k = mb.k;
-  p.ef = mb.ef;
-  p.filter = mb.filter;
-  p.query_filter = mb.dqf;
-  p.selectivity = mb.selectivity;
-  p.out_labels = mb.gl;
-  p.out_dists = mb.gd;
-  p.out_found = mb.gfound;
-  p.out_stats = mb.gstats;
+  MultiGroup g;
+  g.n = n_over;
+  g.filtered = true;
+  g.s = mb.selectivity;
+  SearchParams p = walk_params(h, mb, g, tables, false, nullptr);
   p.qmap = dmap;
   if (mb.timing && h->opt_timing) cudaEventRecord(h->ev[2], h->stream);
   ANNB_TRY(launch_search(h, p, 2));
@@ -1255,6 +1281,193 @@ static int finish_batch(annb_index *h, MultiBatch &mb, bool flagged, bool check)
   return ANNB_OK;
 }
 
+// Enqueue a planned batch on h->stream with the scratch of `lane` (lane 0 also serves the blocking calls): stage and
+// normalise the queries -- gathered into the groups' row order when the batch has a row map (gathered row i is the
+// caller's row (*perm)[i], with bitmap (*qf)[i]) --, run K1 for the groups whose walk does not build its tables (or
+// take the caller's `tables`: one group, not fused), build the label list's bitmap, launch one walk per non-empty group,
+// then scatter the outputs back to the caller's rows and copy them out (batch_outputs).  A blocking call uses the
+// handle's own found slot, work counter and pinned slot 2; it times K1 (ev[0], ev[1]; a gathered batch times its K1
+// with its walks) and its walks (ev[2], ev[3]), dumps its tables (opt_dump_tables) and, in the caller's row order,
+// leaves them to a re-run.  *flagged = some walk can flag queries for a re-run.
+static int enqueue_batch(annb_index *h, int lane, bool blocking, const float *queries, const float *tables, int in_space, int64_t B,
+                         int normalize, int k, int ef_eff, const MultiGroup *grp, int n_grp, const std::vector<uint32_t> *perm,
+                         const std::vector<const uint32_t *> *qf, const uint64_t *filter_labels, int filter_space, int64_t n_filter,
+                         const uint32_t *filter_bits, uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out,
+                         MultiBatch &mb, bool *flagged) {
+  const bool host_in = in_space != ANNB_DEVICE, host_out = out_space != ANNB_DEVICE, gathered = perm != nullptr;
+  const size_t TS = (size_t)h->M * h->Ks, dim = (size_t)h->dim;
+  bool need_tables = false;
+  *flagged = false;
+  for (int i = 0; i < n_grp; i++) {
+    need_tables |= grp[i].n && !grp[i].fuse;
+    *flagged |= grp[i].n && grp[i].mode == 1;
+  }
+  mb = MultiBatch();
+  mb.B = B;
+  mb.k = k;
+  mb.ef = ef_eff;
+  mb.selectivity = gathered ? 1.f : (float)grp[0].s;
+  mb.dl = labels_out;
+  mb.dd = dists_out;
+  mb.gstats = stats_out;
+  mb.table_slot = lane ? S_L1_TABLES : S_TABLES;
+  // all scratch first: a (re)allocation synchronises both lanes, which is only safe before enqueuing
+  if (host_out) {
+    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_L : S_OUT_L, (size_t)B * k * 8, (void **)&mb.dl));
+    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_D : S_OUT_D, (size_t)B * k * 4, (void **)&mb.dd));
+    if (stats_out) ANNB_TRY(annb_scratch(h, S_STATS, (size_t)B * 24, (void **)&mb.gstats));
+    mb.host_labels = labels_out;
+    mb.host_dists = dists_out;
+    mb.host_stats = stats_out;
+  }
+  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t o_perm = al((size_t)B * 8), o_found = o_perm + al((size_t)B * 4), o_gl = o_found + al((size_t)B * 4),
+               o_gd = o_gl + al((size_t)B * k * 8), o_q = o_gd + al((size_t)B * k * 4), total = o_q + al((size_t)B * dim * 4);
+  uint8_t *mq = nullptr;  // a gathered batch: bitmaps, row map, found, outputs and queries, in the gathered order
+  if (gathered) {
+    ANNB_TRY(annb_scratch(h, lane ? S_MULTI1 : S_MULTI0, total, (void **)&mq));
+    mb.dqf = reinterpret_cast<const uint32_t *const *>(mq);
+    mb.dperm = reinterpret_cast<const uint32_t *>(mq + o_perm);
+    mb.gfound = reinterpret_cast<int32_t *>(mq + o_found);
+    mb.gl = reinterpret_cast<uint64_t *>(mq + o_gl);
+    mb.gd = reinterpret_cast<float *>(mq + o_gd);
+  } else {
+    ANNB_TRY(annb_scratch(h, blocking ? S_FOUND : (lane ? S_L1_FOUND : S_L0_FOUND), (size_t)B * 4, (void **)&mb.gfound));
+    mb.gl = mb.dl;
+    mb.gd = mb.dd;
+  }
+  float *dq = nullptr, *dtab = const_cast<float *>(tables);  // device queries are read in place unless normalised
+  if (queries && (host_in || (normalize > 0 && !gathered)))
+    ANNB_TRY(annb_scratch(h, lane ? S_L1_QUERIES : S_QUERIES, (size_t)B * dim * 4, (void **)&dq));
+  if (need_tables && (!tables || host_in)) ANNB_TRY(annb_scratch(h, lane ? S_L1_TABLES : S_TABLES, (size_t)B * TS * 4, (void **)&dtab));
+  uint32_t *by_id = const_cast<uint32_t *>(filter_bits), *by_label = nullptr;
+  uint64_t *staged = nullptr;
+  if (filter_labels) {
+    ANNB_TRY(annb_scratch(h, lane ? S_L1_FLT_BY_ID : S_FLT_BY_ID, ((size_t)(h->gd.n + 31) / 32 + 1) * 4, (void **)&by_id));
+    ANNB_TRY(label_staging(h, lane, filter_space, n_filter, &staged, &by_label));
+  }
+  mb.filter = by_id;
+  unsigned int *counter = nullptr;  // blocking: the handle's own (walk_counter)
+  if (!blocking) {
+    ANNB_TRY(annb_scratch(h, S_LANE_COUNTERS, 512, (void **)&counter));
+    counter += 64 * lane;
+  }
+  ANNB_TRY(annb_pinned(h, blocking ? 2 : 4 + lane, (size_t)B * 4, (void **)&mb.hfound));
+
+  const bool timing = blocking && h->opt_timing, time_k1 = timing && !gathered && need_tables && !tables;
+  if (time_k1) cudaEventRecord(h->ev[0], h->stream);
+  if (gathered) {
+    std::vector<uint8_t> meta(o_found, 0);
+    memcpy(meta.data(), qf->data(), (size_t)B * 8);
+    memcpy(meta.data() + o_perm, perm->data(), (size_t)B * 4);
+    ANNB_CUDA(cudaMemcpyAsync(mq, meta.data(), o_found, cudaMemcpyHostToDevice, h->stream));
+  }
+  if (queries) {
+    const float *src = queries;
+    if (dq) {
+      ANNB_CUDA(cudaMemcpyAsync(dq, queries, (size_t)B * dim * 4, host_in ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice,
+                                h->stream));
+      src = dq;
+    }
+    if (gathered) {
+      ANNB_TRY(launch_rows_copy(h, src, mq + o_q, mb.dperm, B, (int)dim, false));
+      src = reinterpret_cast<float *>(mq + o_q);
+    }
+    for (int r = 0; r < normalize; r++) ANNB_TRY(launch_l2_normalize(h, const_cast<float *>(src), B, (int)dim));
+    mb.dq = src;
+  } else if (host_in) {
+    ANNB_CUDA(cudaMemcpyAsync(dtab, tables, (size_t)B * TS * 4, cudaMemcpyHostToDevice, h->stream));
+  }
+  if (timing && gathered) cudaEventRecord(h->ev[2], h->stream);
+  for (int i = 0; i < n_grp && !tables; i++)
+    if (grp[i].n && !grp[i].fuse) ANNB_TRY(launch_adc_table(h, mb.dq + grp[i].o * dim, grp[i].n, dtab + grp[i].o * TS));
+  if (time_k1) cudaEventRecord(h->ev[1], h->stream);
+  if (filter_labels) ANNB_TRY(labels_to_bitmap(h, filter_labels, filter_space, n_filter, staged, by_label, by_id));
+  if (timing && !gathered) cudaEventRecord(h->ev[2], h->stream);
+  for (int i = 0; i < n_grp; i++)
+    if (grp[i].n) ANNB_TRY(launch_search(h, walk_params(h, mb, grp[i], dtab, blocking && !gathered, counter), grp[i].mode));
+  if (timing) cudaEventRecord(h->ev[3], h->stream);
+  ANNB_TRY(batch_outputs(h, mb));
+  if (blocking && !gathered) {
+    mb.tables = need_tables ? dtab : nullptr;
+    mb.timing = true;
+  }
+  return ANNB_OK;
+}
+
+// The host-buffer plain search as a pipeline of nch chunks on two streams: H2D of chunk c+1 overlaps the walk of chunk
+// c, the walk of chunk c+1 fills the SMs that chunk c's persistent launch leaves idle in its tail, and D2H of chunk c
+// overlaps the walk of chunk c+1.
+static int search_chunked(annb_index *h, const float *queries, int64_t B, int normalize, int k, int ef_eff, bool fuse, int nch,
+                          uint64_t *labels_out, float *dists_out, int64_t *stats_out) {
+  const size_t TS = (size_t)h->M * h->Ks;
+  MultiBatch mb;
+  mb.k = k;
+  mb.ef = ef_eff;
+  float *dq, *dtab = nullptr;
+  unsigned int *counters;
+  int32_t *hfound;
+  ANNB_TRY(annb_scratch(h, S_OUT_L, (size_t)B * k * 8, (void **)&mb.gl));
+  ANNB_TRY(annb_scratch(h, S_OUT_D, (size_t)B * k * 4, (void **)&mb.gd));
+  ANNB_TRY(annb_scratch(h, S_FOUND, (size_t)B * 4, (void **)&mb.gfound));
+  if (stats_out) ANNB_TRY(annb_scratch(h, S_STATS, (size_t)B * 24, (void **)&mb.gstats));
+  ANNB_TRY(annb_scratch(h, S_QUERIES, (size_t)B * h->dim * sizeof(float), (void **)&dq));
+  if (!fuse) ANNB_TRY(annb_scratch(h, S_TABLES, (size_t)B * TS * sizeof(float), (void **)&dtab));
+  ANNB_TRY(annb_scratch(h, S_COUNTER, 256 * 9, (void **)&counters));
+  ANNB_TRY(annb_pinned(h, 2, (size_t)B * 4, (void **)&hfound));
+  mb.dq = dq;
+  ANNB_CUDA(cudaStreamSynchronize(h->stream));  // scratch (re)allocation and earlier work are settled
+  cudaStream_t lanes[2] = {h->stream, h->stream2};
+  cudaStream_t saved = h->stream;
+  int rc = ANNB_OK;
+  for (int c = 0; c < nch && rc == ANNB_OK; c++) {
+    MultiGroup g;
+    g.o = B * c / nch;
+    g.n = B * (c + 1) / nch - g.o;
+    g.fuse = fuse;
+    const int64_t b0 = g.o, nb = g.n;
+    h->stream = lanes[c & 1];
+    if (cudaMemcpyAsync(dq + b0 * h->dim, queries + b0 * h->dim, (size_t)nb * h->dim * sizeof(float),
+                        cudaMemcpyHostToDevice, h->stream) != cudaSuccess) {
+      rc = ANNB_ECUDA;
+      break;
+    }
+    for (int r = 0; r < normalize && rc == ANNB_OK; r++) rc = launch_l2_normalize(h, dq + b0 * h->dim, nb, h->dim);
+    if (rc == ANNB_OK && !fuse) rc = launch_adc_table(h, dq + b0 * h->dim, nb, dtab + b0 * TS);
+    if (rc != ANNB_OK) break;
+    if (c == 0 && h->opt_timing) cudaEventRecord(h->ev[2], h->stream);
+    rc = launch_search(h, walk_params(h, mb, g, dtab, true, counters + 64 * (c + 1)), g.mode);
+    if (rc != ANNB_OK) break;
+    if (c == nch - 1 && h->opt_timing) cudaEventRecord(h->ev[3], h->stream);
+    cudaMemcpyAsync(hfound + b0, mb.gfound + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, h->stream);
+    cudaMemcpyAsync(labels_out + b0 * k, mb.gl + b0 * k, (size_t)nb * k * 8, cudaMemcpyDeviceToHost, h->stream);
+    cudaMemcpyAsync(dists_out + b0 * k, mb.gd + b0 * k, (size_t)nb * k * 4, cudaMemcpyDeviceToHost, h->stream);
+    if (stats_out) cudaMemcpyAsync(stats_out + b0 * 3, mb.gstats + b0 * 3, (size_t)nb * 24, cudaMemcpyDeviceToHost, h->stream);
+  }
+  h->stream = saved;
+  cudaError_t e1 = cudaStreamSynchronize(h->stream), e2 = cudaStreamSynchronize(h->stream2);
+  if (rc != ANNB_OK) {
+    if (rc == ANNB_ECUDA) annb_set_error("CUDA error in the chunked search pipeline: %s", cudaGetErrorString(cudaGetLastError()));
+    return rc;
+  }
+  if (e1 != cudaSuccess || e2 != cudaSuccess)
+    ANNB_FAIL(ANNB_ECUDA, "CUDA error %s in the chunked search pipeline", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+  for (int64_t b = 0; b < B; b++)
+    if (hfound[b] < k)
+      ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
+  return ANNB_OK;
+}
+
+// the one group of a batch under one filter that admits n_filter rows (filtered), or under none
+static MultiGroup single_group(const annb_index *h, int64_t B, int ef_eff, bool filtered, int64_t n_filter) {
+  MultiGroup g;
+  g.n = B;
+  g.filtered = filtered;
+  g.s = search_selectivity(h, filtered, n_filter);
+  g.mode = search_route(h, ef_eff, filtered, g.s, &g.fuse, nullptr);
+  return g;
+}
+
 static int search_impl(annb_index *h, const float *queries, const float *tables, int in_space, int64_t B, int normalize,
                        int k, int ef, const uint64_t *filter_labels, int filter_space, int64_t n_filter,
                        const PreparedFilter *pf, uint64_t *labels_out, float *dists_out, int out_space, int64_t *stats_out) {
@@ -1268,167 +1481,23 @@ static int search_impl(annb_index *h, const float *queries, const float *tables,
   if (B == 0) return ANNB_OK;
   const int ef_eff = std::max(ef, k);  // hnswalg.h:1279
   if (ef_eff > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, k)=%d exceeds ANNB_MAX_EF=%d", ef_eff, ANNB_MAX_EF);
-  const bool host_out = out_space != ANNB_DEVICE;
-  uint64_t *dl = labels_out;
-  float *dd = dists_out;
-  int64_t *dstats = nullptr;
-  int32_t *dfound;
-  if (host_out) {
-    ANNB_TRY(annb_scratch(h, S_OUT_L, (size_t)B * k * 8, (void **)&dl));
-    ANNB_TRY(annb_scratch(h, S_OUT_D, (size_t)B * k * 4, (void **)&dd));
-  }
-  ANNB_TRY(annb_scratch(h, S_FOUND, (size_t)B * 4, (void **)&dfound));
-  if (stats_out) {
-    if (host_out) ANNB_TRY(annb_scratch(h, S_STATS, (size_t)B * 24, (void **)&dstats));
-    else dstats = stats_out;
-  }
   if (h->gd.n == 0) {  // empty index: searchKnn returns nothing (hnswalg.h:1240)
     ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   }
-  // ---- host-buffer fast path: chunked two-stream pipeline -------------------------------------------
-  // H2D of chunk c+1 overlaps the walk of chunk c, the walk of chunk c+1 fills the SMs that chunk c's
-  // persistent launch leaves idle in its tail, and D2H of chunk c overlaps the walk of chunk c+1.
-  {
-    const bool plain = !has_filter && h->g.num_deleted == 0 && !h->opt_force_general;
-    int nch = (int)h->opt_chunks;
-    if (nch == 0) nch = (B >= 32768) ? 4 : (B >= 4096 ? 2 : 1);
-    if (nch > 8) nch = 8;
-    if (queries && in_space != ANNB_DEVICE && host_out && plain && nch > 1 && B >= 2 * nch) {
-      const size_t TS = (size_t)h->M * h->Ks;
-      // the walk builds its own tables (or, wide rows, needs none): no (B,M,Ks) buffer at all
-      const bool fuse = walk4_can_fuse(h) || wide_rows(h);
-      float *dq, *dtab = nullptr;
-      unsigned int *counters;
-      int32_t *hfound;
-      ANNB_TRY(annb_scratch(h, S_QUERIES, (size_t)B * h->dim * sizeof(float), (void **)&dq));
-      if (!fuse) ANNB_TRY(annb_scratch(h, S_TABLES, (size_t)B * TS * sizeof(float), (void **)&dtab));
-      ANNB_TRY(annb_scratch(h, S_COUNTER, 256 * 9, (void **)&counters));
-      ANNB_TRY(annb_pinned(h, 2, (size_t)B * 4, (void **)&hfound));
-      if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
-      ANNB_CUDA(cudaStreamSynchronize(h->stream));  // scratch (re)allocation and earlier work are settled
-      cudaStream_t lanes[2] = {h->stream, h->stream2};
-      cudaStream_t saved = h->stream;
-      int rc = ANNB_OK;
-      for (int c = 0; c < nch && rc == ANNB_OK; c++) {
-        const int64_t b0 = B * c / nch, b1 = B * (c + 1) / nch, nb = b1 - b0;
-        h->stream = lanes[c & 1];
-        if (cudaMemcpyAsync(dq + b0 * h->dim, queries + b0 * h->dim, (size_t)nb * h->dim * sizeof(float),
-                            cudaMemcpyHostToDevice, h->stream) != cudaSuccess) {
-          rc = ANNB_ECUDA;
-          break;
-        }
-        for (int r = 0; r < normalize && rc == ANNB_OK; r++) rc = launch_l2_normalize(h, dq + b0 * h->dim, nb, h->dim);
-        if (rc == ANNB_OK && !fuse) rc = launch_adc_table(h, dq + b0 * h->dim, nb, dtab + b0 * TS);
-        if (rc != ANNB_OK) break;
-        SearchParams p;
-        memset(&p, 0, sizeof(p));
-        if (fuse) fuse_params(h, p, dq + b0 * h->dim);
-        else p.tables = dtab + b0 * TS;
-        if (h->opt_dump_tables) p.dump_tables = reinterpret_cast<float *>(h->opt_dump_tables) + b0 * TS;
-        p.B = nb;
-        p.k = k;
-        p.ef = ef_eff;
-        p.out_labels = dl + b0 * k;
-        p.out_dists = dd + b0 * k;
-        p.out_found = dfound + b0;
-        p.out_stats = dstats ? dstats + b0 * 3 : nullptr;
-        p.work_counter = counters + 64 * (c + 1);
-        if (c == 0 && h->opt_timing) cudaEventRecord(h->ev[2], h->stream);
-        rc = launch_search(h, p, false);
-        if (rc != ANNB_OK) break;
-        if (c == nch - 1 && h->opt_timing) cudaEventRecord(h->ev[3], h->stream);
-        cudaMemcpyAsync(hfound + b0, dfound + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, h->stream);
-        cudaMemcpyAsync(labels_out + b0 * k, dl + b0 * k, (size_t)nb * k * 8, cudaMemcpyDeviceToHost, h->stream);
-        cudaMemcpyAsync(dists_out + b0 * k, dd + b0 * k, (size_t)nb * k * 4, cudaMemcpyDeviceToHost, h->stream);
-        if (stats_out) cudaMemcpyAsync(stats_out + b0 * 3, dstats + b0 * 3, (size_t)nb * 24, cudaMemcpyDeviceToHost, h->stream);
-      }
-      h->stream = saved;
-      cudaError_t e1 = cudaStreamSynchronize(h->stream), e2 = cudaStreamSynchronize(h->stream2);
-      if (rc != ANNB_OK) {
-        if (rc == ANNB_ECUDA) annb_set_error("CUDA error in the chunked search pipeline: %s", cudaGetErrorString(cudaGetLastError()));
-        return rc;
-      }
-      if (e1 != cudaSuccess || e2 != cudaSuccess)
-        ANNB_FAIL(ANNB_ECUDA, "CUDA error %s in the chunked search pipeline", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
-      for (int64_t b = 0; b < B; b++)
-        if (hfound[b] < k)
-          ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
-      return ANNB_OK;
-    }
-  }
-  // tables: handed in (the literal dtables argument), built inside the walk (plain search, hnsw_walk4), or by K1
-  const size_t tbytes = (size_t)B * h->M * h->Ks * sizeof(float);
-  const float *dt = nullptr, *dq_fused = nullptr;
-  const bool plain_search = !has_filter && h->g.num_deleted == 0 && !h->opt_force_general;
-  // fraction of the nodes a filtered / deletion-aware walk can admit: sizes its lists
-  const double selectivity = has_filter ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
-                                           : 1.0 - (double)h->g.num_deleted / (double)std::max<int64_t>(1, h->gd.n);
-  // the table is built inside the walk for the plain search (hnsw_walk4) and for the filtered one (hnsw_walk4f)
-  // (hnsw_walk_wide computes its distances from the queries in every mode)
-  const bool fuse_walk = wide_rows(h) ||
-                         (walk4_can_fuse(h) && (plain_search || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, selectivity))));
-  if (tables) {
-    ANNB_TRY(stage_in(h, tables, in_space, tbytes, S_TABLES, (const void **)&dt));
-  } else if (fuse_walk) {
-    ANNB_TRY(stage_queries(h, queries, in_space, B, normalize, S_QUERIES, &dq_fused));
-  } else {
-    float *t;
-    ANNB_TRY(annb_scratch(h, S_TABLES, tbytes, (void **)&t));
-    ANNB_TRY(build_tables(h, queries, in_space, B, normalize, t));
-    dt = t;
-  }
-  // filter
-  const uint32_t *dfilter = nullptr;
-  if (pf) {
-    dfilter = pf->bits;
-  } else if (filter_labels) {
-    uint32_t *by_id, *by_label;
-    uint64_t *staged;
-    ANNB_TRY(annb_scratch(h, S_FLT_BY_ID, ((size_t)(h->gd.n + 31) / 32 + 1) * 4, (void **)&by_id));
-    ANNB_TRY(label_staging(h, 0, filter_space, n_filter, &staged, &by_label));
-    ANNB_TRY(labels_to_bitmap(h, filter_labels, filter_space, n_filter, staged, by_label, by_id));
-    dfilter = by_id;
-  }
-  SearchParams p;
-  memset(&p, 0, sizeof(p));
-  if (dq_fused) fuse_params(h, p, dq_fused);
-  else p.tables = dt;
-  if (h->opt_dump_tables) p.dump_tables = reinterpret_cast<float *>(h->opt_dump_tables);
-  p.B = B;
-  p.k = k;
-  p.ef = ef_eff;
-  p.filter = dfilter;
-  p.out_labels = dl;
-  p.out_dists = dd;
-  p.out_found = dfound;
-  p.out_stats = dstats;
-  const bool general = dfilter != nullptr || h->g.num_deleted > 0 || h->opt_force_general;
-  p.selectivity = (float)selectivity;
+  if (queries && !h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
+  MultiGroup g = single_group(h, B, ef_eff, has_filter, n_filter);
+  g.fuse &= !tables;  // the caller's tables: the walk reads them
+  int nch = (int)h->opt_chunks;
+  if (nch == 0) nch = (B >= 32768) ? 4 : (B >= 4096 ? 2 : 1);
+  if (nch > 8) nch = 8;
+  if (queries && in_space != ANNB_DEVICE && out_space != ANNB_DEVICE && g.mode == 0 && nch > 1 && B >= 2 * nch)
+    return search_chunked(h, queries, B, normalize, k, ef_eff, g.fuse, nch, labels_out, dists_out, stats_out);
   MultiBatch mb;
-  mb.B = B;
-  mb.k = k;
-  mb.ef = ef_eff;
-  mb.dq = p.queries;
-  mb.filter = dfilter;
-  mb.selectivity = p.selectivity;
-  mb.gl = mb.dl = dl;
-  mb.gd = mb.dd = dd;
-  mb.gfound = dfound;
-  mb.gstats = dstats;
-  mb.host_labels = host_out ? labels_out : nullptr;
-  mb.host_dists = host_out ? dists_out : nullptr;
-  mb.host_stats = host_out ? stats_out : nullptr;
-  mb.tables = p.tables;
-  mb.table_slot = S_TABLES;
-  mb.timing = true;
-  ANNB_TRY(annb_pinned(h, 2, (size_t)B * 4, (void **)&mb.hfound));
-  const int mode = general ? (h->opt_force_general == 2 ? 2 : 1) : 0;
-  if (h->opt_timing) cudaEventRecord(h->ev[2], h->stream);
-  ANNB_TRY(launch_search(h, p, mode));
-  if (h->opt_timing) cudaEventRecord(h->ev[3], h->stream);
-  ANNB_TRY(batch_outputs(h, mb));
+  bool flagged;
+  ANNB_TRY(enqueue_batch(h, 0, true, queries, tables, in_space, B, normalize, k, ef_eff, &g, 1, nullptr, nullptr, filter_labels,
+                         filter_space, n_filter, pf ? pf->bits : nullptr, labels_out, dists_out, out_space, stats_out, mb, &flagged));
   ANNB_CUDA(cudaStreamSynchronize(h->stream));
-  return finish_batch(h, mb, mode != 2, true);
+  return finish_batch(h, mb, flagged, true);
 }
 
 extern "C" {
@@ -1524,11 +1593,15 @@ static int lane_wait(annb_index *h, int lane) {
   return lane_finish(h, lane, true);
 }
 
-// one batch, enqueued entirely on one lane: H2D -> normalise -> [filter bitmap] -> walk (tables built inside) -> D2H
-// The filter is a label list or a prepared bitmap (pf), as in search_impl.
+static int multi_plan(annb_index *h, int64_t B, int ef_eff, const int *query_filter, std::vector<uint32_t> &perm,
+                      std::vector<const uint32_t *> &qf, MultiGroup grp[3]);
+
+// one batch, enqueued entirely on the next ticket's lane (enqueue_batch) once that lane's previous batch is done.  The
+// filter is a label list or a prepared bitmap (pf), as in search_impl, or one prepared filter per query (query_filter),
+// as in annb_search_multi.
 static int submit_impl(annb_index *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
                        const uint64_t *filter_labels, int filter_space, int64_t n_filter, const PreparedFilter *pf,
-                       uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
+                       const int *query_filter, uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
   if (pf) n_filter = pf->count;
   if (!queries || !labels_out || !dists_out || !ticket_out || B <= 0 || k <= 0 || ef <= 0) ANNB_FAIL(ANNB_EINVAL, "bad arguments");
   if (n_filter < 0 || (n_filter > 0 && !filter_labels && !pf)) ANNB_FAIL(ANNB_EINVAL, "bad filter");
@@ -1543,89 +1616,25 @@ static int submit_impl(annb_index *h, const float *queries, int in_space, int64_
   if (h->gd.n == 0) ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   const int ef_eff = std::max(ef, k);
   if (ef_eff > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, k)=%d exceeds ANNB_MAX_EF=%d", ef_eff, ANNB_MAX_EF);
-  const bool general = filter_labels != nullptr || pf || h->g.num_deleted > 0 || h->opt_force_general;
-  const double selectivity = (filter_labels || pf) ? std::min<double>(1.0, (double)n_filter / (double)std::max<int64_t>(1, h->gd.n))
-                                                   : 1.0 - (double)h->g.num_deleted / (double)std::max<int64_t>(1, h->gd.n);
+  std::vector<uint32_t> perm;
+  std::vector<const uint32_t *> qf;
+  MultiGroup grp[3];
+  if (query_filter) ANNB_TRY(multi_plan(h, B, ef_eff, query_filter, perm, qf, grp));
+  else grp[0] = single_group(h, B, ef_eff, filter_labels || pf, n_filter);
   const int ticket = (int)(h->next_ticket++ & 0x3fffffff);
   const int lane = ticket & 1;
   ANNB_TRY(lane_wait(h, lane));  // a lane holds one batch at a time
-  const bool host_in = in_space != ANNB_DEVICE, host_out = out_space != ANNB_DEVICE;
-  const size_t TS = (size_t)h->M * h->Ks;
-  const bool fuse = wide_rows(h) || (walk4_can_fuse(h) && (!general || walk4f_applicable(h, ef_eff, selectivity)));
-  float *dq = nullptr, *dtab = nullptr, *dd = dists_out;
-  uint64_t *dl = labels_out;
-  int32_t *dfound;
-  unsigned int *counters;
-  uint32_t *by_id = pf ? pf->bits : nullptr, *by_label = nullptr;
-  uint64_t *dflt = nullptr;
-  // all scratch first: a (re)allocation synchronises both lanes, which is only safe before enqueuing
-  if (host_in || normalize > 0)
-    ANNB_TRY(annb_scratch(h, lane ? S_L1_QUERIES : S_QUERIES, (size_t)B * h->dim * sizeof(float), (void **)&dq));
-  if (!fuse) ANNB_TRY(annb_scratch(h, lane ? S_L1_TABLES : S_TABLES, (size_t)B * TS * sizeof(float), (void **)&dtab));
-  if (host_out) {
-    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_L : S_OUT_L, (size_t)B * k * 8, (void **)&dl));
-    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_D : S_OUT_D, (size_t)B * k * 4, (void **)&dd));
-  }
-  ANNB_TRY(annb_scratch(h, lane ? S_L1_FOUND : S_L0_FOUND, (size_t)B * 4, (void **)&dfound));
-  ANNB_TRY(annb_scratch(h, S_LANE_COUNTERS, 512, (void **)&counters));
-  if (filter_labels) {
-    ANNB_TRY(annb_scratch(h, lane ? S_L1_FLT_BY_ID : S_FLT_BY_ID, ((size_t)(h->gd.n + 31) / 32 + 1) * 4, (void **)&by_id));
-    ANNB_TRY(label_staging(h, lane, filter_space, n_filter, &dflt, &by_label));
-  }
-  MultiBatch mb;
-  ANNB_TRY(annb_pinned(h, 4 + lane, (size_t)B * 4, (void **)&mb.hfound));
-  mb.B = B;
-  mb.k = k;
-  mb.ef = ef_eff;
-  mb.filter = by_id;
-  mb.selectivity = (float)selectivity;
-  mb.gl = mb.dl = dl;
-  mb.gd = mb.dd = dd;
-  mb.gfound = dfound;
-  mb.host_labels = host_out ? labels_out : nullptr;
-  mb.host_dists = host_out ? dists_out : nullptr;
-  mb.table_slot = lane ? S_L1_TABLES : S_TABLES;
-
+  annb_index::AsyncLane &L = h->lanes[lane];
   cudaStream_t saved = h->stream;
   h->stream = lane ? h->stream2 : saved;
-  int rc = ANNB_OK;
-  const float *src = queries;
-  if (dq) {
-    if (cudaMemcpyAsync(dq, queries, (size_t)B * h->dim * sizeof(float), host_in ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice,
-                        h->stream) != cudaSuccess)
-      rc = ANNB_ECUDA;
-    src = dq;
-  }
-  mb.dq = src;
-  for (int r = 0; r < normalize && rc == ANNB_OK; r++) rc = launch_l2_normalize(h, dq, B, h->dim);
-  if (rc == ANNB_OK && filter_labels) rc = labels_to_bitmap(h, filter_labels, filter_space, n_filter, dflt, by_label, by_id);
-  if (rc == ANNB_OK && !fuse) rc = launch_adc_table(h, src, B, dtab);
-  if (rc == ANNB_OK) {
-    SearchParams p;
-    memset(&p, 0, sizeof(p));
-    if (fuse) fuse_params(h, p, src);
-    else p.tables = dtab;
-    p.B = B;
-    p.k = k;
-    p.ef = ef_eff;
-    p.filter = by_id;
-    p.out_labels = dl;
-    p.out_dists = dd;
-    p.out_found = dfound;
-    p.work_counter = counters + 64 * lane;
-    p.selectivity = (float)selectivity;
-    rc = launch_search(h, p, general ? 1 : 0);
-  }
-  if (rc == ANNB_OK) rc = batch_outputs(h, mb);
+  bool flagged = false;
+  const int rc = enqueue_batch(h, lane, false, queries, nullptr, in_space, B, normalize, k, ef_eff, grp, query_filter ? 3 : 1,
+                               query_filter ? &perm : nullptr, query_filter ? &qf : nullptr, filter_labels, filter_space, n_filter,
+                               pf ? pf->bits : nullptr, labels_out, dists_out, out_space, nullptr, L.batch, &flagged);
   h->stream = saved;
-  if (rc != ANNB_OK) {
-    if (rc == ANNB_ECUDA) annb_set_error("CUDA error while enqueuing a streamed search");
-    return rc;
-  }
-  annb_index::AsyncLane &L = h->lanes[lane];
+  if (rc != ANNB_OK) return rc;
   L.busy = true;
-  L.flagged = general;
-  L.batch = mb;
+  L.flagged = flagged;
   *ticket_out = ticket;
   return ANNB_OK;
 }
@@ -1634,8 +1643,8 @@ int annb_search_submit(annb_index_t *h, const float *queries, int in_space, int6
                        uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
-  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, nullptr, labels_out, dists_out, out_space,
-                     ticket_out);
+  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, nullptr, nullptr, labels_out, dists_out,
+                     out_space, ticket_out);
 }
 
 int annb_search_submit_filtered(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
@@ -1644,8 +1653,8 @@ int annb_search_submit_filtered(annb_index_t *h, const float *queries, int in_sp
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
   if (!filter_labels && n_filter != 0) ANNB_FAIL(ANNB_EINVAL, "bad filter");
-  return submit_impl(h, queries, in_space, B, normalize, k, ef, filter_labels, filter_space, n_filter, nullptr, labels_out, dists_out,
-                     out_space, ticket_out);
+  return submit_impl(h, queries, in_space, B, normalize, k, ef, filter_labels, filter_space, n_filter, nullptr, nullptr, labels_out,
+                     dists_out, out_space, ticket_out);
 }
 
 int annb_search_wait(annb_index_t *h, int ticket) {
@@ -2306,31 +2315,20 @@ int annb_search_submit_prepared(annb_index_t *h, const float *queries, int in_sp
   ANNB_NEED_GPU(h);
   PreparedFilter *f;
   ANNB_TRY(find_filter(h, filter_id, &f));
-  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, f, labels_out, dists_out, out_space, ticket_out);
+  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, f, nullptr, labels_out, dists_out, out_space,
+                     ticket_out);
 }
 
 // ---- per-query filters ----------------------------------------------------------------------------------
-// A batch with one filter per query is split into three routing groups, each ONE launch over its rows gathered into a
-// contiguous block: 0 = no filter (the plain walk, or the deletion-aware one), 1 = filters hnsw_walk4f takes (its list
-// N sized by the group's smallest selectivity, so one selective filter does not move every query to the round-1
-// kernel), 2 = the other filtered rows (hnsw_walk_flagged / the bitmap walk).  Each walk reads query q's bitmap from
+// A batch with one filter per query is split into three routing groups (MultiGroup), gathered into contiguous blocks,
+// each on the route annb_search_prepared / annb_search take for the same rows.  Each walk reads query q's bitmap from
 // the per-query table; queries any walk flagged are re-run on the bitmap walk with their own bitmap.
-struct MultiGroup {
-  int64_t o = 0, n = 0;  // gathered rows [o, o + n)
-  bool filtered = false;
-  double s = 1.0;        // the selectivity the group's lists are sized by
-  int mode = 0;          // launch_search mode
-  bool fuse = false;     // tables built inside the walk (else K1 first)
-};
-
-// the route annb_search_prepared / annb_search take for the same rows, group by group
 static int multi_plan(annb_index *h, int64_t B, int ef_eff, const int *query_filter, std::vector<uint32_t> &perm,
                       std::vector<const uint32_t *> &qf, MultiGroup grp[3]) {
-  const double nn = (double)std::max<int64_t>(1, h->gd.n);
   std::unordered_map<int, std::pair<const PreparedFilter *, int>> seen;  // id -> (filter, group)
   std::vector<int8_t> which((size_t)B);
   std::vector<const uint32_t *> bits((size_t)B, nullptr);
-  double smin[3] = {1.0, 1.0, 1.0};
+  double smin[3] = {search_selectivity(h, false, 0), 1.0, 1.0};
   int64_t cnt[3] = {0, 0, 0};
   for (int64_t b = 0; b < B; b++) {
     const int id = query_filter[b];
@@ -2340,8 +2338,10 @@ static int multi_plan(annb_index *h, int64_t B, int ef_eff, const int *query_fil
       if (it == seen.end()) {
         PreparedFilter *pf;
         ANNB_TRY(find_filter(h, id, &pf));
-        const double s = std::min<double>(1.0, (double)pf->count / nn);
-        g = (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, s)) ? 1 : 2;
+        const double s = search_selectivity(h, true, pf->count);
+        bool walk4f;
+        search_route(h, ef_eff, true, s, nullptr, &walk4f);
+        g = walk4f ? 1 : 2;
         smin[g] = std::min(smin[g], s);
         it = seen.emplace(id, std::make_pair((const PreparedFilter *)pf, g)).first;
       }
@@ -2357,117 +2357,16 @@ static int multi_plan(annb_index *h, int64_t B, int ef_eff, const int *query_fil
   for (int g = 0; g < 3; g++) {
     grp[g].o = at[g];
     grp[g].n = cnt[g];
+    grp[g].filtered = g > 0;
+    grp[g].s = smin[g];
+    grp[g].mode = search_route(h, ef_eff, g > 0, smin[g], &grp[g].fuse, nullptr);
   }
   for (int64_t b = 0; b < B; b++) {
     const int64_t pos = at[which[(size_t)b]]++;
     perm[(size_t)pos] = (uint32_t)b;
     qf[(size_t)pos] = bits[(size_t)b];
   }
-  const bool can_fuse = walk4_can_fuse(h);
-  {  // no filter: search_impl with filter_labels == NULL
-    MultiGroup &g = grp[0];
-    const bool general = h->g.num_deleted > 0 || h->opt_force_general;
-    g.s = 1.0 - (double)h->g.num_deleted / nn;
-    g.mode = general ? (h->opt_force_general == 2 ? 2 : 1) : 0;
-    g.fuse = wide_rows(h) || (can_fuse && (!general || (h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s))));
-  }
-  for (int i = 1; i < 3; i++) {  // a prepared filter: the filtered route
-    MultiGroup &g = grp[i];
-    g.filtered = true;
-    g.s = smin[i];
-    g.mode = h->opt_force_general == 2 ? 2 : 1;
-    g.fuse = wide_rows(h) || (can_fuse && h->opt_force_general != 2 && walk4f_applicable(h, ef_eff, g.s));
-  }
   return ANNB_OK;
-}
-
-// Enqueue a planned batch on h->stream with the scratch of `lane` (0 also serves the blocking call): gather the
-// queries, normalise, one walk per group, scatter the outputs back to the caller's rows, copy `found` (gathered order)
-// and host outputs back.  *flagged = some walk may have flagged queries for a re-run.
-static int multi_enqueue(annb_index *h, int lane, const float *queries, int in_space, int64_t B, int normalize, int k, int ef_eff,
-                         const std::vector<uint32_t> &perm, const std::vector<const uint32_t *> &qf, const MultiGroup grp[3],
-                         uint64_t *labels_out, float *dists_out, int out_space, int pinned_slot, unsigned int *counters,
-                         bool timing, MultiBatch &mb, bool *flagged) {
-  const bool host_in = in_space != ANNB_DEVICE, host_out = out_space != ANNB_DEVICE;
-  const size_t TS = (size_t)h->M * h->Ks, dim = (size_t)h->dim;
-  bool need_tables = false;
-  *flagged = false;
-  for (int g = 0; g < 3; g++) {
-    if (grp[g].n && !grp[g].fuse) need_tables = true;
-    if (grp[g].n && grp[g].mode != 0) *flagged = true;
-  }
-  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
-  const size_t o_perm = al((size_t)B * 8), o_found = o_perm + al((size_t)B * 4), o_gl = o_found + al((size_t)B * 4),
-               o_gd = o_gl + al((size_t)B * k * 8), o_q = o_gd + al((size_t)B * k * 4), total = o_q + al((size_t)B * dim * 4);
-  // all scratch first: a (re)allocation synchronises both lanes, which is only safe before enqueuing
-  uint8_t *mq;
-  ANNB_TRY(annb_scratch(h, lane ? S_MULTI1 : S_MULTI0, total, (void **)&mq));
-  float *draw = nullptr, *dtab = nullptr;
-  if (host_in) ANNB_TRY(annb_scratch(h, lane ? S_L1_QUERIES : S_QUERIES, (size_t)B * dim * 4, (void **)&draw));
-  if (need_tables) ANNB_TRY(annb_scratch(h, lane ? S_L1_TABLES : S_TABLES, (size_t)B * TS * 4, (void **)&dtab));
-  uint64_t *dl = labels_out;
-  float *dd = dists_out;
-  if (host_out) {
-    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_L : S_OUT_L, (size_t)B * k * 8, (void **)&dl));
-    ANNB_TRY(annb_scratch(h, lane ? S_L1_OUT_D : S_OUT_D, (size_t)B * k * 4, (void **)&dd));
-  }
-  int32_t *hfound;
-  ANNB_TRY(annb_pinned(h, pinned_slot, (size_t)B * 4, (void **)&hfound));
-  std::vector<uint8_t> meta(o_found, 0);
-  memcpy(meta.data(), qf.data(), (size_t)B * 8);
-  memcpy(meta.data() + o_perm, perm.data(), (size_t)B * 4);
-  mb = MultiBatch();
-  mb.B = B;
-  mb.k = k;
-  mb.ef = ef_eff;
-  mb.dqf = reinterpret_cast<const uint32_t *const *>(mq);
-  mb.dperm = reinterpret_cast<const uint32_t *>(mq + o_perm);
-  mb.gfound = reinterpret_cast<int32_t *>(mq + o_found);
-  mb.gl = reinterpret_cast<uint64_t *>(mq + o_gl);
-  mb.gd = reinterpret_cast<float *>(mq + o_gd);
-  float *dq = reinterpret_cast<float *>(mq + o_q);
-  mb.dq = dq;
-  mb.dl = dl;
-  mb.dd = dd;
-  mb.host_labels = host_out ? labels_out : nullptr;
-  mb.host_dists = host_out ? dists_out : nullptr;
-  mb.hfound = hfound;
-  mb.table_slot = lane ? S_L1_TABLES : S_TABLES;
-
-  int rc = ANNB_OK;
-  const float *src = queries;
-  if (cudaMemcpyAsync(mq, meta.data(), o_found, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) rc = ANNB_ECUDA;
-  if (rc == ANNB_OK && host_in) {
-    if (cudaMemcpyAsync(draw, queries, (size_t)B * dim * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) rc = ANNB_ECUDA;
-    src = draw;
-  }
-  if (rc == ANNB_OK) rc = launch_rows_copy(h, src, dq, mb.dperm, B, (int)dim, false);
-  for (int r = 0; r < normalize && rc == ANNB_OK; r++) rc = launch_l2_normalize(h, dq, B, (int)dim);
-  if (rc == ANNB_OK && timing) cudaEventRecord(h->ev[2], h->stream);
-  for (int gi = 0; gi < 3 && rc == ANNB_OK; gi++) {
-    const MultiGroup &g = grp[gi];
-    if (g.n == 0) continue;
-    if (!g.fuse) rc = launch_adc_table(h, dq + g.o * dim, g.n, dtab + g.o * TS);
-    if (rc != ANNB_OK) break;
-    SearchParams p;
-    memset(&p, 0, sizeof(p));
-    if (g.fuse) fuse_params(h, p, dq + g.o * dim);
-    else p.tables = dtab + g.o * TS;
-    p.B = g.n;
-    p.k = k;
-    p.ef = ef_eff;
-    p.query_filter = g.filtered ? mb.dqf + g.o : nullptr;
-    p.selectivity = (float)g.s;
-    p.out_labels = mb.gl + g.o * k;
-    p.out_dists = mb.gd + g.o * k;
-    p.out_found = mb.gfound + g.o;
-    p.work_counter = counters;
-    rc = launch_search(h, p, g.mode);
-  }
-  if (rc == ANNB_OK && timing) cudaEventRecord(h->ev[3], h->stream);
-  if (rc == ANNB_OK) rc = batch_outputs(h, mb);
-  if (rc == ANNB_ECUDA) annb_set_error("CUDA error while enqueuing a per-query filter search: %s", cudaGetErrorString(cudaGetLastError()));
-  return rc;
 }
 
 int annb_search_multi(annb_index_t *h, const float *queries, int in_space, int64_t B, int normalize, int k, int ef,
@@ -2489,9 +2388,9 @@ int annb_search_multi(annb_index_t *h, const float *queries, int in_space, int64
   ANNB_TRY(multi_plan(h, B, ef_eff, query_filter, perm, qf, grp));
   if (h->gd.n == 0) ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
   MultiBatch mb;
-  bool flagged = false;
-  ANNB_TRY(multi_enqueue(h, 0, queries, in_space, B, normalize, k, ef_eff, perm, qf, grp, labels_out, dists_out, out_space, 2,
-                         nullptr, h->opt_timing != 0, mb, &flagged));
+  bool flagged;
+  ANNB_TRY(enqueue_batch(h, 0, true, queries, nullptr, in_space, B, normalize, k, ef_eff, grp, 3, &perm, &qf, nullptr, ANNB_HOST, 0,
+                         nullptr, labels_out, dists_out, out_space, nullptr, mb, &flagged));
   ANNB_CUDA(cudaStreamSynchronize(h->stream));
   return finish_batch(h, mb, flagged, true);
 }
@@ -2500,40 +2399,9 @@ int annb_search_submit_multi(annb_index_t *h, const float *queries, int in_space
                              const int *query_filter, uint64_t *labels_out, float *dists_out, int out_space, int *ticket_out) {
   ANNB_ENTER(h);
   ANNB_NEED_GPU(h);
-  if (!queries || !query_filter || !labels_out || !dists_out || !ticket_out || B <= 0 || k <= 0 || ef <= 0)
-    ANNB_FAIL(ANNB_EINVAL, "bad arguments");
-  if (!h->g.inited) ANNB_FAIL(ANNB_ESTATE, "index not initialised");
-  if (!h->d_codebook) ANNB_FAIL(ANNB_ESTATE, "Please train the PQ before using HNSW quantization backend");
-  if (h->opt_force_general == 2) ANNB_FAIL(ANNB_EINVAL, "streamed searches do not run on the bitmap walk: use annb_search");
-  if (h->dev_dirty || h->deleted_dirty || h->patch_pending) {  // re-upload of the graph: nothing may be in flight
-    ANNB_TRY(lane_wait(h, 0));
-    ANNB_TRY(lane_wait(h, 1));
-    ANNB_TRY(sync_device_graph(h));
-  }
-  if (h->gd.n == 0) ANNB_FAIL(ANNB_EFEWRESULTS, "Cannot return the results in a contigious 2D array. Probably ef or M is too small");
-  const int ef_eff = std::max(ef, k);
-  if (ef_eff > ANNB_MAX_EF) ANNB_FAIL(ANNB_ELIMIT, "max(ef, k)=%d exceeds ANNB_MAX_EF=%d", ef_eff, ANNB_MAX_EF);
-  std::vector<uint32_t> perm;
-  std::vector<const uint32_t *> qf;
-  MultiGroup grp[3];
-  ANNB_TRY(multi_plan(h, B, ef_eff, query_filter, perm, qf, grp));
-  const int ticket = (int)(h->next_ticket++ & 0x3fffffff);
-  const int lane = ticket & 1;
-  ANNB_TRY(lane_wait(h, lane));  // a lane holds one batch at a time
-  unsigned int *counters;
-  ANNB_TRY(annb_scratch(h, S_LANE_COUNTERS, 512, (void **)&counters));
-  annb_index::AsyncLane &L = h->lanes[lane];
-  cudaStream_t saved = h->stream;
-  h->stream = lane ? h->stream2 : saved;
-  bool flagged = false;
-  const int rc = multi_enqueue(h, lane, queries, in_space, B, normalize, k, ef_eff, perm, qf, grp, labels_out, dists_out, out_space,
-                               4 + lane, counters + 64 * lane, false, L.batch, &flagged);
-  h->stream = saved;
-  if (rc != ANNB_OK) return rc;
-  L.busy = true;
-  L.flagged = flagged;
-  *ticket_out = ticket;
-  return ANNB_OK;
+  if (!query_filter) ANNB_FAIL(ANNB_EINVAL, "bad arguments");
+  return submit_impl(h, queries, in_space, B, normalize, k, ef, nullptr, ANNB_HOST, 0, nullptr, query_filter, labels_out, dists_out,
+                     out_space, ticket_out);
 }
 
 }  // extern "C"

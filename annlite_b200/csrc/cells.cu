@@ -944,7 +944,7 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
       kc[c] = (int32_t)std::min<int64_t>({(int64_t)limit, f->count, std::max<int64_t>(live, 0)});
       bits[c] = f->bits;
       // the selectivity annb_search_prepared sizes the cell's lists by (SearchParams::selectivity is fp32)
-      sel[c] = (float)std::min<double>(1.0, (double)f->count / (double)std::max<int64_t>(1, h->gd.n));
+      sel[c] = (float)search_selectivity(h, true, f->count);
       pfs[c] = f;
       bool sc;
       ANNB_TRY_RC(scan_decision(cs, c, f, true, exact, own_codes, &sc));
@@ -968,7 +968,7 @@ int annb_cellset_search_prepared(annb_cellset_t *cs, const float *queries, int i
         n_own++;
       }
     }
-    if (ep == 4 && en > 0) en = en <= 4 ? 4 : (en <= 6 ? 6 : 8);
+    if (en > 0) en = walk4f_round_en(ep, en);
   }
   cs->last_route = fused ? 0 : 1;
   cs->last_rerun_pairs = 0;
@@ -1133,14 +1133,13 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
     ndel[c] = h->g.num_deleted;
     const int64_t live = std::max<int64_t>(h->g.count.load() - h->g.num_deleted, 0);
     nlive[c] = live;
-    const double nn = (double)std::max<int64_t>(1, h->gd.n);
     std::unordered_map<int, const PreparedFilter *> pf;
     for (int64_t s = 0; s < S; s++) {
       const int id = row_id(s, c);
       const size_t i = (size_t)(s * C + c);
       if (id == 0) {  // annb_search_multi's unfiltered rows: the live rows (k = min(limit, live), container.py:119)
         sk[i] = (int32_t)std::min<int64_t>(limit, live);
-        ssel[i] = (float)(1.0 - (double)h->g.num_deleted / nn);
+        ssel[i] = (float)search_selectivity(h, false, 0);
         if (exact && sk[i] > 0) {  // ANNB_CELLS_EXACT: scanned over the cell's live rows
           sscan[i] = 1;
           ANNB_TRY_RC(scan_cell(cs, c, own_codes));
@@ -1162,7 +1161,7 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       const PreparedFilter *f = it->second;
       sk[i] = (int32_t)std::min<int64_t>({(int64_t)limit, f->count, live});
       sbits[i] = f->bits;
-      ssel[i] = (float)std::min<double>(1.0, (double)f->count / nn);
+      ssel[i] = (float)search_selectivity(h, true, f->count);
       spf[i] = f;
       bool sc;
       ANNB_TRY_RC(scan_decision(cs, c, f, false, exact, own_codes, &sc));
@@ -1225,7 +1224,7 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       if (fused && walk4f_geometry(cs->cells[c], std::max(ef, sk[i]), (double)ssel[i], &ep_c, &en_c)) en = std::max(en, en_c);
       else own[i] = 1;
     }
-  if (ep == 4 && en > 0) en = en <= 4 ? 4 : (en <= 6 ? 6 : 8);
+  if (en > 0) en = walk4f_round_en(ep, en);
   StagedScans ss;
   ANNB_TRY_RC(stage_scans(cs, plans, own_codes, gd, !fused, ss));
   if (!plans.empty()) ANNB_TRY_RC(batch_tables(cs, b, B));
@@ -1277,7 +1276,9 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
       const size_t i = (size_t)slot[(size_t)q] * C + c;
       if (!walked[(size_t)(q * C + c)] || !own[i]) continue;
       const int k = sk[i];
-      const int kind = !sbits[i] ? 0 : ((h->opt_force_general != 2 && walk4f_applicable(h, std::max(ef, k), ssel[i])) ? 1 : 2);
+      bool walk4f = false;
+      if (sbits[i]) search_route(h, std::max(ef, k), true, ssel[i], nullptr, &walk4f);
+      const int kind = !sbits[i] ? 0 : (walk4f ? 1 : 2);
       Group &g = groups[{k, kind}];
       g.rows.push_back((uint32_t)q);
       if (kind) g.qf.push_back(sbits[i]);
@@ -1285,8 +1286,7 @@ int annb_cellset_search_multi(annb_cellset_t *cs, const float *queries, int in_s
     }
     for (auto &kv : groups) {
       const int k = kv.first.first, kind = kv.first.second;
-      int mode = h->opt_force_general == 2 ? 2 : 1;
-      if (kind == 0 && ndel[c] == 0 && !h->opt_force_general) mode = 0;
+      const int mode = search_route(h, std::max(ef, k), kind != 0, kv.second.s, nullptr, nullptr);
       ANNB_TRY_RC(own_launch(cs, b, B, limit, ef, c, mode, k, (float)kv.second.s, nullptr, kv.second.rows, kv.second.qf, true));
     }
     if (!groups.empty()) cs->last_handle_cells++;

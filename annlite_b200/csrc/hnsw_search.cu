@@ -1285,6 +1285,21 @@ int launch_search(annb_index *h, const SearchParams &p, int mode) {
   });
 }
 
+int search_route(const annb_index *h, int ef, bool filtered, double selectivity, bool *fuse, bool *walk4f) {
+  const bool general = filtered || h->g.num_deleted > 0 || h->opt_force_general;
+  const int mode = !general ? 0 : (h->opt_force_general == 2 ? 2 : 1);
+  const bool w4f = mode == 1 && walk4f_applicable(h, ef, selectivity);
+  // launch_search builds no tables: a walk without them must be one that builds its own (hnsw_walk_wide always does)
+  if (fuse) *fuse = wide_rows(h) || (walk4_can_fuse(h) && (mode == 0 || w4f));
+  if (walk4f) *walk4f = w4f;
+  return mode;
+}
+
+double search_selectivity(const annb_index *h, bool filtered, int64_t count) {
+  const double n = (double)std::max<int64_t>(1, h->gd.n);
+  return filtered ? std::min<double>(1.0, (double)count / n) : 1.0 - (double)h->g.num_deleted / n;
+}
+
 int walk_counter(annb_index *h, SearchParams &p) {
   if (!p.work_counter) ANNB_TRY_RC(annb_scratch(h, 4, 256, (void **)&p.work_counter));
   ANNB_CUDA(cudaMemsetAsync(p.work_counter, 0, 8, h->stream));

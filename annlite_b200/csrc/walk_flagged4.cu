@@ -471,11 +471,11 @@ bool walk4f_geometry(const annb_index *h, int ef, double selectivity, int *ep_ou
   int en = walk4f_en_for(ef, selectivity);
   if (h->opt_flagged_en >= 2 && h->opt_flagged_en <= 8 && h->opt_flagged_en != 7) en = (int)h->opt_flagged_en;  // tests / A-B: force N's size
   if (en == 0) return false;
-  if (ep == 4) en = en <= 4 ? 4 : (en <= 6 ? 6 : 8);
   *ep_out = ep;
-  *en_out = en;
+  *en_out = walk4f_round_en(ep, en);
   return true;
 }
+int walk4f_round_en(int ep, int en) { return ep == 4 ? (en <= 4 ? 4 : (en <= 6 ? 6 : 8)) : en; }
 bool walk4f_applicable(const annb_index *h, int ef, double selectivity) {
   int ep, en;
   return walk4f_geometry(h, ef, selectivity, &ep, &en);
